@@ -112,9 +112,7 @@ __global__ void __launch_bounds__(256) flow_code_d8_x4_kernel(const float *__res
     }
     *reinterpret_cast<uchar4 *>(code + i0) = make_uchar4(cd[0], cd[1], cd[2], cd[3]);
     double *ap = accum + i0;
-    if (ones == 2) {
-      // packed unit-weight path: deps_gather_packed_x4_kernel initialises the accumulator words
-    } else if (ones) {
+    if (ones) {
       reinterpret_cast<double2 *>(ap)[0] = make_double2(cd[0] == kCodeNoData ? -1.0 : 1.0, cd[1] == kCodeNoData ? -1.0 : 1.0);
       reinterpret_cast<double2 *>(ap)[1] = make_double2(cd[2] == kCodeNoData ? -1.0 : 1.0, cd[3] == kCodeNoData ? -1.0 : 1.0);
     } else {
@@ -609,8 +607,9 @@ __global__ void sanitize_dirs_kernel(const uint8_t *__restrict__ dirs, uint8_t *
 }  // namespace
 
 // =================================================================================================
-// Unit-weight D8 (the Python default, richdem.FlowAccumulation(dem, 'D8')): every partial sum is an
-// integer < 2^31, so a cell's accumulator and its remaining-donor count share ONE 64-bit word
+// Unit-weight D8 over row bands (the single-GPU path, fa_d8_tiles below, uses the same protocol on shared memory
+// inside 64 x 64 tiles): every partial sum is an integer < 2^31, so a cell's accumulator and its remaining-donor count
+// share ONE 64-bit word
 //     [ 8 bits donors left | 56 bits integer sum ]
 // living in the caller's accumulation array.  A donor adds (value - 1<<56) with a single atomicAdd:
 // the returned old word tells it whether it was the last donor, and if so the complete sum -- no
@@ -1586,37 +1585,303 @@ __global__ void __launch_bounds__(256) band_apply_packed_kernel(unsigned long lo
     row[x] = (left << 56) | val;
   }
 }
+
+// =================================================================================================
+// Unit-weight D8 on one GPU, tile by tile: the perimeter method of Barnes (2017) for out-of-core D8 accumulation
+// (the reference's programs/parallel_d8_accum) with shared memory as the "core".  The raster is cut into 64 x 64
+// tiles; the cells on a tile's edge are its *slots*.  Almost every D8 path is short, so almost all the work stays in
+// shared memory and only the flow that crosses tile edges goes through a small global solve:
+//   1. fa_tile_codes_kernel: per tile, the flow codes from the DEM window (tile + one-cell apron) -> code bytes
+//      (tile-major scratch), then the in-tile accumulation of unit flow.  Per slot it records in `link`: for an
+//      *exit* slot (receiver in another tile) the receiver's slot, for any other slot the exit slot of the same tile
+//      where its in-tile path leaves the tile (or none), and in `lword` the exit slot's local accumulation.
+//   2. fa_link_count_kernel + fa_link_walk_kernel: exit slot p drains into next(p), the exit slot where the in-tile
+//      path from its receiver's slot leaves that tile.  The exit slots form a forest, solved by the packed countdown
+//      walk over slots; each exit's total outflow is added to the inflow of its receiver's slot.
+//   3. fa_tile_final_kernel: per tile, the codes again, every cell seeded with 1 plus the inflow on its slot, the same
+//      in-tile accumulation, the result written as doubles.
+// Per cell, HBM sees 4 B (DEM) + 2 x 1 B (codes) + 8 B (result); per slot (1/16 of the cells) 16 B of link data.  No
+// global atomic touches the cell raster.  All sums are integers < 2^31, so the result is exact whatever the order.
+// =================================================================================================
+constexpr int kFaT = 64;                           // tile side
+constexpr int kFaCells = kFaT * kFaT;
+constexpr int kFaSlots = 4 * kFaT;                 // slot numbers per tile: top row, bottom row, left, right column
+constexpr unsigned long long kLkOne = 1ull << 32;  // link words: [32 bits donors left | 32 bits sum]; an exit slot can
+                                                   // have hundreds of donors, more than the 8-bit field of kPkOne holds
+
+// width (height) of a tile that starts `left` columns (rows) before the raster's edge
+__device__ __forceinline__ int fa_side(int left) { return left < kFaT ? left : kFaT; }
+
+// slot of the edge cell (lx, ly) of a tw x th tile, -1 for an inner cell (a corner belongs to its row)
+__device__ __forceinline__ int fa_slot_of(int lx, int ly, int tw, int th) {
+  if (ly == 0) return lx;
+  if (ly == th - 1) return kFaT + lx;
+  if (lx == 0) return 2 * kFaT + ly;
+  if (lx == tw - 1) return 3 * kFaT + ly;
+  return -1;
+}
+
+// the cell of slot s; false where s names no cell of a tw x th tile
+__device__ __forceinline__ bool fa_slot_cell(int s, int tw, int th, int &lx, int &ly) {
+  const int k = s & (kFaT - 1), side = s / kFaT;
+  if (side < 2) {
+    lx = k;
+    ly = side == 0 ? 0 : th - 1;
+    return k < tw && (side == 0 || th > 1);
+  }
+  lx = side == 2 ? 0 : tw - 1;
+  ly = k;
+  return k > 0 && k < th - 1 && (side == 2 || tw > 1);
+}
+
+// In-tile unit-weight accumulation in shared memory.  sCode: the tile's codes (row stride kFaT; kCodeNoData for NoData
+// and for cells beyond the raster), sWord: each data cell's seed, sQueue: room for the tile's sources and two counters
+// that are zero on entry.  Afterwards every data cell's word holds its seed plus the seeds of its upstream cells inside
+// the tile: the countdown protocol of the packed walk above, on shared memory.  The sources (cells without a donor in
+// the tile, listed before any walk can complete a cell) go into one queue per tile, and a thread whose walk has ended
+// takes the next one, so that a warp's time is about its share of the steps rather than the sum of its longest walks.
+__device__ __forceinline__ void fa_tile_accumulate(const uint8_t *sCode, unsigned long long *sWord, uint16_t *sQueue,
+                                                   int *sCount, int tw, int th) {
+  const int t = threadIdx.x;
+  for (int k = 0; k < kFaCells / 256; k++) {
+    const int c = t + 256 * k, lx = c & (kFaT - 1), ly = c / kFaT;
+    if (sCode[c] == kCodeNoData) continue;
+    unsigned deps = 0;
+#pragma unroll
+    for (int n = 1; n <= 8; n++) {
+      const int x = lx + d8dx(n), y = ly + d8dy(n);
+      if (x >= 0 && y >= 0 && x < tw && y < th && (sCode[y * kFaT + x] & 15) == d8_inverse(n)) deps++;
+    }
+    if (deps) sWord[c] += (unsigned long long)deps << 56;
+    else sQueue[atomicAdd(&sCount[0], 1)] = (uint16_t)c;
+  }
+  __syncthreads();
+  const int nsrc = sCount[0];
+  int cur = 0;
+  unsigned long long acc = 0;
+  bool walking = false;
+  for (;;) {  // one walk step per iteration, so that the lanes of a warp stay together
+    if (!walking) {
+      const int i = atomicAdd(&sCount[1], 1);
+      if (i >= nsrc) break;
+      cur = sQueue[i];
+      acc = sWord[cur];
+      walking = true;
+    }
+    const int d = sCode[cur] & 15;
+    const int x = (cur & (kFaT - 1)) + d8dx(d), y = cur / kFaT + d8dy(d);
+    if (d == 0 || x < 0 || y < 0 || x >= tw || y >= th) {  // no receiver, or it is in another tile
+      walking = false;
+      continue;
+    }
+    const int r = y * kFaT + x;
+    const unsigned long long old = atomicAdd(&sWord[r], acc - kPkOne);
+    if ((old >> 56) != 1ull) {  // other donors are still to come: the last one carries on
+      walking = false;
+      continue;
+    }
+    acc = (old & kPkVal) + acc;
+    cur = r;
+  }
+  __syncthreads();
+}
+
+__global__ void __launch_bounds__(256) fa_tile_codes_kernel(const float *__restrict__ dem, uint8_t *__restrict__ code,
+                                                             int *__restrict__ link, unsigned long long *__restrict__ lword,
+                                                             unsigned *__restrict__ inflow, int W, int H, float nodata,
+                                                             int tiles_x) {
+  constexpr int kWin = kFaT + 2;  // DEM window: the tile and a one-cell apron
+  static_assert(kWin * kWin * sizeof(float) <= kFaCells * sizeof(unsigned long long), "the DEM window lives in sWord");
+  __shared__ __align__(16) unsigned long long sWord[kFaCells];  // first the DEM window, then the accumulation words
+  __shared__ __align__(16) uint8_t sCode[kFaCells];
+  __shared__ uint16_t sQueue[kFaCells];
+  __shared__ int sCount[2];
+  const int t = threadIdx.x, tile = blockIdx.x;
+  if (t < 2) sCount[t] = 0;
+  const int bx = tile % tiles_x, by = tile / tiles_x;
+  const int x0 = bx * kFaT, y0 = by * kFaT;
+  const int tw = fa_side(W - x0), th = fa_side(H - y0);
+  float *sDem = reinterpret_cast<float *>(sWord);
+  for (int i = t; i < kWin * kWin; i += 256) {
+    const int wy = i / kWin, wx = i - wy * kWin;
+    const int gy = y0 - 1 + wy, gx = x0 - 1 + wx;
+    sDem[i] = (gy >= 0 && gy < H && gx >= 0 && gx < W) ? __ldg(dem + (size_t)gy * W + gx) : nodata;
+  }
+  __syncthreads();
+  // flow codes, the rule of fa_d8_prep_rolling_kernel: the first strictly lowest data neighbour; raster-border cells have
+  // no receiver.  Thread t: column t % 64, a strip of 16 rows, a rolling 3 x 3 register window.
+  {
+    const int lx = t & (kFaT - 1), ly0 = (t / kFaT) * (kFaT / 4);
+    float a[3][3];
+#pragma unroll
+    for (int j = 1; j < 3; j++)
+#pragma unroll
+      for (int k = 0; k < 3; k++) a[j][k] = sDem[(ly0 + j - 1) * kWin + lx + k];
+    for (int j = 0; j < kFaT / 4; j++) {
+      const int ly = ly0 + j;
+#pragma unroll
+      for (int k = 0; k < 3; k++) {
+        a[0][k] = a[1][k];
+        a[1][k] = a[2][k];
+        a[2][k] = sDem[(ly + 2) * kWin + lx + k];
+      }
+      const float e = a[1][1];
+      const int gx = x0 + lx, gy = y0 + ly;
+      int cd = 0;
+      if (lx >= tw || ly >= th || e == nodata) {
+        cd = kCodeNoData;
+      } else if (!(gx == 0 || gy == 0 || gx == W - 1 || gy == H - 1)) {
+        // neighbours n = 1..8 : W, NW, N, NE, E, SE, S, SW.  Starting the running minimum at the cell's own value folds
+        // the reference's `>= e` skip into it (capped at FLT_MAX, the reference's starting value)
+        const float ne[9] = {0.f, a[1][0], a[0][0], a[0][1], a[0][2], a[1][2], a[2][2], a[2][1], a[2][0]};
+        float lowest = fminf(e, 3.402823466e+38f);
+#pragma unroll
+        for (int n = 1; n <= 8; n++) {
+          const float v = ne[n];
+          if (v < lowest && v != nodata) {
+            lowest = v;
+            cd = n;
+          }
+        }
+      }
+      sCode[ly * kFaT + lx] = (uint8_t)cd;
+    }
+  }
+  __syncthreads();  // the DEM window is dead from here on
+  reinterpret_cast<uint4 *>(code + (size_t)tile * kFaCells)[t] = reinterpret_cast<const uint4 *>(sCode)[t];
+  for (int c = t; c < kFaCells; c += 256) sWord[c] = 1;
+  fa_tile_accumulate(sCode, sWord, sQueue, sCount, tw, th);
+  // ---- per slot (one per thread): where its in-tile path leaves the tile ----
+  const size_t gs = (size_t)tile * kFaSlots + t;
+  int lk = -1;  // -1: the path ends inside the tile (or the slot is NoData / unused)
+  unsigned long long out = 0;
+  int lx, ly;
+  if (fa_slot_cell(t, tw, th, lx, ly) && sCode[ly * kFaT + lx] != kCodeNoData) {
+    int cur = ly * kFaT + lx;
+    for (;;) {
+      const int d = sCode[cur] & 15;
+      if (d == 0) break;
+      const int cx = cur & (kFaT - 1), cy = cur / kFaT;
+      const int x = cx + d8dx(d), y = cy + d8dy(d);
+      if (x < 0 || y < 0 || x >= tw || y >= th) {
+        if (cur == ly * kFaT + lx) {  // an exit slot: link to the receiver's slot (encoded as -2 - slot)
+          const int gx = x0 + x, gy = y0 + y, rbx = gx / kFaT, rby = gy / kFaT;
+          const int rs = fa_slot_of(gx - rbx * kFaT, gy - rby * kFaT, fa_side(W - rbx * kFaT), fa_side(H - rby * kFaT));
+          lk = -2 - ((rby * tiles_x + rbx) * kFaSlots + rs);
+          out = kLkOne | (sWord[cur] & kPkVal);  // the count starts at 1: the slot's own token (fa_link_walk_kernel)
+        } else {
+          lk = tile * kFaSlots + fa_slot_of(cx, cy, tw, th);
+        }
+        break;
+      }
+      cur = y * kFaT + x;
+    }
+  }
+  link[gs] = lk;
+  lword[gs] = out;
+  inflow[gs] = 0;
+}
+
+// the exit slot where the in-tile path from slot r leaves its tile, -1 if it ends inside
+__device__ __forceinline__ int fa_link_next(const int *link, int r) {
+  const int l = link[r];
+  return l <= -2 ? r : l;
+}
+
+__global__ void __launch_bounds__(256) fa_link_count_kernel(const int *__restrict__ link, unsigned long long *lword,
+                                                             int nslots) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= nslots) return;
+  const int l = link[p];
+  if (l > -2) return;  // not an exit slot
+  const int q = fa_link_next(link, -2 - l);
+  if (q >= 0) atomicAdd(&lword[q], kLkOne);
+}
+
+// Every exit slot delivers its own token first: the party that brings a count to zero -- the slot itself when all its
+// donors have arrived, else its last donor -- owns the total and walks on.  Its outflow goes to the receiver's inflow.
+__global__ void __launch_bounds__(256) fa_link_walk_kernel(const int *__restrict__ link, unsigned long long *lword,
+                                                            unsigned *inflow, int nslots) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= nslots) return;
+  int l = link[p];
+  if (l > -2) return;
+  const unsigned long long old = atomicAdd(&lword[p], 0ull - kLkOne);
+  if ((old >> 32) != 1ull) return;
+  unsigned long long acc = old & (kLkOne - 1);
+  for (;;) {
+    const int r = -2 - l;
+    atomicAdd(&inflow[r], (unsigned)acc);
+    const int q = fa_link_next(link, r);
+    if (q < 0) break;
+    const unsigned long long o = atomicAdd(&lword[q], acc - kLkOne);
+    if ((o >> 32) != 1ull) break;
+    acc = (o & (kLkOne - 1)) + acc;
+    l = link[q];
+  }
+}
+
+__global__ void __launch_bounds__(256) fa_tile_final_kernel(const uint8_t *__restrict__ code,
+                                                             const unsigned *__restrict__ inflow, double *__restrict__ accum,
+                                                             int W, int H, int tiles_x) {
+  __shared__ __align__(16) unsigned long long sWord[kFaCells];
+  __shared__ __align__(16) uint8_t sCode[kFaCells];
+  __shared__ uint16_t sQueue[kFaCells];
+  __shared__ int sCount[2];
+  const int t = threadIdx.x, tile = blockIdx.x;
+  const int bx = tile % tiles_x, by = tile / tiles_x;
+  const int x0 = bx * kFaT, y0 = by * kFaT;
+  const int tw = fa_side(W - x0), th = fa_side(H - y0);
+  if (t < 2) sCount[t] = 0;
+  reinterpret_cast<uint4 *>(sCode)[t] = __ldg(reinterpret_cast<const uint4 *>(code + (size_t)tile * kFaCells) + t);
+  for (int c = t; c < kFaCells; c += 256) sWord[c] = 1;
+  __syncthreads();
+  int lx, ly;
+  if (fa_slot_cell(t, tw, th, lx, ly)) sWord[ly * kFaT + lx] += __ldg(inflow + (size_t)tile * kFaSlots + t);
+  __syncthreads();
+  fa_tile_accumulate(sCode, sWord, sQueue, sCount, tw, th);
+  for (int c = t; c < kFaCells; c += 256) {
+    const int cx = c & (kFaT - 1), cy = c / kFaT;
+    if (cx < tw && cy < th)
+      accum[(size_t)(y0 + cy) * W + x0 + cx] = sCode[c] == kCodeNoData ? -1.0 : (double)(sWord[c] & kPkVal);  // -1: flow_accumulation_generic.hpp:95-97
+  }
+}
+
+// the number of slots fa_d8_tiles needs for a w x h raster (slots are numbered with int)
+long long fa_tile_slots(int w, int h) {
+  return (long long)((w + kFaT - 1) / kFaT) * ((h + kFaT - 1) / kFaT) * kFaSlots;
+}
+
+void fa_d8_tiles(const float *d_dem, double *d_accum, int w, int h, float nodata) {
+  Ctx &c = ctx();
+  const int tiles_x = (w + kFaT - 1) / kFaT;
+  const long long nslots = fa_tile_slots(w, h);
+  const unsigned ntiles = (unsigned)(nslots / kFaSlots);
+  DevBuf<uint8_t> code((size_t)ntiles * kFaCells);
+  DevBuf<int> link((size_t)nslots);
+  DevBuf<unsigned long long> lword((size_t)nslots);
+  DevBuf<unsigned> inflow((size_t)nslots);
+  const unsigned sblocks = (unsigned)((nslots + 255) / 256);
+  fa_tile_codes_kernel<<<ntiles, 256, 0, c.stream>>>(d_dem, code.p, link.p, lword.p, inflow.p, w, h, nodata, tiles_x);
+  fa_link_count_kernel<<<sblocks, 256, 0, c.stream>>>(link.p, lword.p, (int)nslots);
+  KernelTimer kt;
+  fa_link_walk_kernel<<<sblocks, 256, 0, c.stream>>>(link.p, lword.p, inflow.p, (int)nslots);
+  kt.stop_async();
+  fa_tile_final_kernel<<<ntiles, 256, 0, c.stream>>>(code.p, inflow.p, d_accum, w, h, tiles_x);
+  RDB_CK(cudaGetLastError());
+  count_launch(4);
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  c.stats.ms_main_kernel += kt.ms();
+  c.stats.accum_rounds = 1;
+}
 }  // namespace
 
 // FA_D8 / FA_Tarboton fused (reference methods/flow_accumulation.hpp:27,16): no 36 B/cell props
 void fa_fused_dev(const float *d_dem, double *d_accum, int w, int h, float nodata, bool ones, bool dinf) {
   Ctx &c = ctx();
   const size_t n = (size_t)w * h;
-  if (!dinf && ones && (w & 3) == 0 && ((uintptr_t)d_dem & 15) == 0 && ((uintptr_t)d_accum & 15) == 0 &&
-      c.params.accum_packed) {
-    // unit-weight D8: packed integer accumulation (see above)
-    DevBuf<uint8_t> code(n);
-    dim3 blk(256), grd((w / 4 + 255) / 256, h < 8192 ? h : 8192);
-    if (c.params.accum_fused_prep) {
-      dim3 pgrd((unsigned)((w + kPrepOut - 1) / kPrepOut), (unsigned)((h + kPrepRows - 1) / kPrepRows));
-      fa_d8_prep_rolling_kernel<<<pgrd, blk, 0, c.stream>>>(d_dem, code.p, reinterpret_cast<unsigned long long *>(d_accum), w, h,
-                                                            nodata, 0, h);
-      count_launch();
-    } else {
-      flow_code_d8_x4_kernel<<<grd, blk, 0, c.stream>>>(d_dem, code.p, d_accum, w, h, nodata, 2);
-      deps_gather_packed_x4_kernel<<<grd, blk, 0, c.stream>>>(code.p, reinterpret_cast<unsigned long long *>(d_accum), w, h, 0, h);
-      count_launch(2);
-    }
-    RDB_CK(cudaGetLastError());
-    KernelTimer kt;
-    launch_walk_packed<false>(code.p, reinterpret_cast<unsigned long long *>(d_accum), w, (int)n, nullptr, 0, 0,
-                              c.params.accum_fused_prep != 0);
-    RDB_CK(cudaGetLastError());
-    count_launch();
-    kt.stop_async();
-    RDB_CK(cudaStreamSynchronize(c.stream));
-    c.stats.ms_main_kernel += kt.ms();
-    c.stats.accum_rounds = 1;
+  if (!dinf && ones && c.params.accum_packed && fa_tile_slots(w, h) < INT32_MAX) {
+    fa_d8_tiles(d_dem, d_accum, w, h, nodata);  // unit-weight D8: tile by tile (see above)
     return;
   }
   DevBuf<uint8_t> code(n);

@@ -73,14 +73,14 @@ struct Params {
   int64_t flats_tiled = 1;   // flat-resolution gradients by the tile engine (0: one cooperative BFS launch each)
   int64_t accum_dinf_packed = 1;  // unit-weight D-infinity: 0 level-synchronous kernel, 1 packed fixed-point walk in phases, 2 packed only when > 5 % of the cells have no receiver
   int64_t flowmet_tarboton_filter = 1;  // FM_Tarboton: pick the steepest facet from squared slopes first (flowmet.cuh), 0: the reference's sequence for every cell
-  int64_t accum_walk_ahead = 0;   // packed D8 walk: sources a warp keeps queued ahead of its lanes (0: 64; 32..128)
-  int64_t accum_walk_scan = 0;    // packed D8 walk, source scan: 0 over the 8 B words (measured best: 13.1 vs 16.6 ms FA_D8 at 32768^2), 1 over the flagged code bytes + L2 prefetch of the words, 2 without the prefetch
+  int64_t accum_walk_ahead = 0;   // packed D8 walk (row bands): sources a warp keeps queued ahead of its lanes (0: 64; 32..128)
+  int64_t accum_walk_scan = 0;    // packed D8 walk (row bands), source scan: 0 over the 8 B words, 1 over the flagged code bytes + L2 prefetch of the words, 2 without the prefetch
   int64_t accum_dinf_stats = 0;   // packed D-infinity: print what the warps spent their iterations on (diagnostics)
   int64_t accum_dinf_share = -1;  // packed D-infinity: ring entries above which a warp asks for a rebalancing phase once enough warps wait (-1: 1)
   int64_t accum_dinf_wait = 0;    // packed D-infinity: ... once 1 / this share of the warps wait at the barrier (0: 4)
-  int64_t accum_packed = 1;  // unit-weight D8: accumulator and donor count share one 64-bit word
-  int64_t accum_fused_prep = 1;   // unit-weight D8: flow codes + donor counts + sole-donor bits in one rolling-window pass
-  int64_t accum_walk_lanes = 1;   // unit-weight D8 walk: persistent always-busy lanes fed from per-warp source queues
+  int64_t accum_packed = 1;  // unit-weight D8: one GPU by 64 x 64 tiles, row bands on packed words (0: the generic walk)
+  int64_t accum_fused_prep = 1;   // unit-weight D8 (row bands): flow codes + donor counts + sole-donor bits in one rolling-window pass
+  int64_t accum_walk_lanes = 1;   // unit-weight D8 walk (row bands): persistent always-busy lanes fed from per-warp source queues
   int64_t accum_threads = 256;
   int64_t accum_budget = 0;  // cells one thread follows per level in the multi-receiver accumulation (0: 4)
 };
