@@ -279,6 +279,14 @@ RDB200_API int rdb200_mgpu_fill_depressions_d8_f32(const rdb200_comm *comm, floa
 RDB200_API int rdb200_mgpu_fa_f32_f64(const rdb200_comm *comm, const float *d_band_dem, double *d_band_accum_inout,
                                       int32_t width, int32_t local_rows, float nodata, int32_t ghost_top,
                                       int32_t ghost_bottom, int32_t dinf, int32_t accum_is_ones, int32_t *exchange_rounds);
+/* Any FlowAccumulation method over row bands; method numbered as in rdb200_dev_fa_method_f32_f64: 0 FA_D8,
+ * 1 FA_Tarboton, 2 FA_D4, 3 FA_Holmgren (xparam; FA_Quinn = 1.0), 4 FA_Freeman (xparam).  Everything else as
+ * rdb200_mgpu_fa_f32_f64, which is this call with method 0 / 1.  An unknown method, or a non-finite xparam for
+ * methods 3 and 4, is an error. */
+RDB200_API int rdb200_mgpu_fa_method_f32_f64(const rdb200_comm *comm, const float *d_band_dem, double *d_band_accum_inout,
+                                             int32_t width, int32_t local_rows, float nodata, int32_t ghost_top,
+                                             int32_t ghost_bottom, int32_t method, double xparam, int32_t accum_is_ones,
+                                             int32_t *exchange_rounds);
 
 /* ---- row-band (multi-GPU) fill: one band per GPU, halo rows exchanged by the caller -- */
 /* The band raster handed in is (band_rows + ghost rows) x width.  Its first and last rows are
@@ -336,8 +344,15 @@ typedef struct rdb200_facc_state rdb200_facc_state;
 RDB200_API int rdb200_dev_facc_begin(rdb200_facc_state **state, const float *d_dem, double *d_accum_inout,
                                      int32_t width, int32_t height, float nodata, int32_t ghost_top,
                                      int32_t ghost_bottom, int32_t dinf, int32_t accum_is_ones);
+/* rdb200_dev_facc_begin for any method (numbered as in rdb200_mgpu_fa_method_f32_f64); the other rdb200_dev_facc_*
+ * steps work on either kind of state. */
+RDB200_API int rdb200_dev_facc_begin_method(rdb200_facc_state **state, const float *d_dem, double *d_accum_inout,
+                                            int32_t width, int32_t height, float nodata, int32_t ghost_top,
+                                            int32_t ghost_bottom, int32_t method, double xparam, int32_t accum_is_ones);
 /* which: 0 = top side, 1 = bottom side.  Flow codes (1 byte/cell, + float rmax for D-infinity) of
- * my first/last owned row, to be installed as the neighbour's ghost codes. */
+ * my first/last owned row, to be installed as the neighbour's ghost codes.  Methods 2-4 (proportions) send a seam donor
+ * mask in the code bytes instead (bit j: the cell sends a share to the neighbour's column x + j - 1; rmax unused), and
+ * set_ghost_codes adds the shares it announces to the donor counts of my edge row. */
 RDB200_API int rdb200_dev_facc_get_edge_codes(rdb200_facc_state *state, int32_t which, uint8_t *d_code_row,
                                               float *d_rmax_row);
 RDB200_API int rdb200_dev_facc_set_ghost_codes(rdb200_facc_state *state, int32_t which,

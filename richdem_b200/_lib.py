@@ -83,6 +83,7 @@ SIGNATURES = {
     "rdb200_comm_destroy": [_vp],
     "rdb200_mgpu_fill_depressions_d8_f32": [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
     "rdb200_mgpu_fa_f32_f64": [_vp, _vp, _vp, _i32, _i32, _f32, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_mgpu_fa_method_f32_f64": [_vp, _vp, _vp, _i32, _i32, _f32, _i32, _i32, _i32, C.c_double, _i32, C.POINTER(_i32)],
     "rdb200_dev_fill_begin": [C.POINTER(_vp), _vp, _i32, _i32],
     "rdb200_dev_fill_begin_lifted": [C.POINTER(_vp), _vp, _i32, _i32, _vp, _i32, _i32, _i32],
     "rdb200_dev_maxpool_rows_f32": [_vp, _i32, _i32, _i32, _i32, _vp, _i32, _i32],
@@ -94,6 +95,7 @@ SIGNATURES = {
     "rdb200_dev_fill_update_row": [_vp, _i32, _vp],
     "rdb200_dev_fill_finish": [_vp, _vp],
     "rdb200_dev_facc_begin": [C.POINTER(_vp), _vp, _vp, _i32, _i32, _f32, _i32, _i32, _i32, _i32],
+    "rdb200_dev_facc_begin_method": [C.POINTER(_vp), _vp, _vp, _i32, _i32, _f32, _i32, _i32, _i32, C.c_double, _i32],
     "rdb200_dev_facc_get_edge_codes": [_vp, _i32, _vp, _vp],
     "rdb200_dev_facc_set_ghost_codes": [_vp, _i32, _vp, _vp],
     "rdb200_dev_facc_run": [_vp, C.POINTER(_i32), C.POINTER(_i32)],

@@ -13,6 +13,7 @@
 // independent of the order in which atomics land (bit-identical to the serial reference).
 #include "flowmet.cuh"
 
+#include <cmath>
 #include <cooperative_groups.h>
 namespace cg = cooperative_groups;
 
@@ -456,6 +457,8 @@ __device__ __forceinline__ void levels_follow(const WalkArgs<double> &a, int c, 
           if (pk <= 0) continue;  // generic.hpp:82-83
           const int r = c + d8dy(k) * W + d8dx(k);
           if (a.props[(size_t)9 * r] == kNoDataGen) continue;  // :85-86
+          // row bands: a share bound for a ghost cell is parked there as one parcel
+          if (BAND && park_in_ghost(a, r, (double)pk * acc)) continue;
           atomicAdd(a.accum + r, (double)pk * acc);
           sent |= 1u << k;
         }
@@ -489,7 +492,7 @@ __device__ __forceinline__ void levels_follow(const WalkArgs<double> &a, int c, 
 // single-file reaches cost no extra levels, while every other cell it completes -- and its own
 // continuation when the budget runs out -- is appended (coalesced-group atomics) to the next
 // frontier, where other threads pick it up in parallel.  Levels meet at grid.sync().
-// BAND (row bands, D-infinity): level 0 can be seeded with the cells completed by a neighbour's flow
+// BAND (row bands, D-infinity and proportions): level 0 can be seeded with the cells completed by a neighbour's flow
 // (q0[0..ncells), seeded != 0) and flow into a ghost row is parked there instead of followed.
 template <int MODE, bool BAND = false>
 __global__ void __launch_bounds__(256) accum_levels_kernel(const WalkArgs<double> a, int *q0, int *q1, int *counts,
@@ -2049,14 +2052,86 @@ __global__ void __launch_bounds__(256) band_zero_ghost_kernel(double *row, int W
   if (x < W) row[x] = 0.0;
 }
 
+// ---- proportions (D4, Quinn, Holmgren, Freeman) over row bands ----
+// The ghost rows are local edge rows, so their proportions carry no flow and they donate to nobody here: flow from the
+// neighbour's edge row into my edge row is announced by a seam donor mask instead, one byte per cell of the sender's
+// edge row.  Bit j (j = 0, 1, 2) set: the cell sends a share across the seam to column x + j - 1, whose cell is not
+// NoData -- exactly the shares the sender's walk parks in its ghost row.
+__global__ void __launch_bounds__(256) band_seam_mask_kernel(const float *__restrict__ props, uint8_t *__restrict__ mask,
+                                                              int W, int row, int dy) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= W) return;
+  uint32_t m = 0;
+  if (x > 0 && x < W - 1) {  // edge columns carry no flow
+    const size_t i = (size_t)row * W + x;
+    const float *p = props + 9 * i;
+    if (p[0] != kNoDataGen) {
+#pragma unroll
+      for (int k = 1; k <= 8; k++) {
+        if (d8dy(k) != dy || !(p[k] > 0)) continue;
+        const size_t r = i + (ptrdiff_t)dy * W + d8dx(k);
+        if (props[9 * r] == kNoDataGen) continue;  // the walk drops flow into NoData
+        m |= 1u << (d8dx(k) + 1);
+      }
+    }
+  }
+  mask[x] = (uint8_t)m;
+}
+
+// my edge row's donor counts += the neighbour's shares that point at each cell
+__global__ void __launch_bounds__(256) band_add_seam_donors_kernel(const uint8_t *__restrict__ mask, uint32_t *st_row, int W) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= W) return;
+  uint32_t k = (mask[x] >> 1) & 1u;               // straight across
+  if (x + 1 < W) k += mask[x + 1] & 1u;            // from x + 1, one column left
+  if (x > 0) k += (mask[x - 1] >> 2) & 1u;         // from x - 1, one column right
+  st_row[x] += k;
+}
+
+// weights: ghost rows become empty parking slots, NoData cells -1 (generic.hpp:95-97), unit weights 1.0
+__global__ void __launch_bounds__(256) band_init_props_accum_kernel(const float *__restrict__ props, double *accum, int W,
+                                                                     int H, int y_lo, int y_hi, int ones) {
+  const size_t n = (size_t)W * H;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int y = (int)(i / W);
+  if (y < y_lo || y >= y_hi) accum[i] = 0.0;
+  else if (props[9 * i] == kNoDataGen) accum[i] = -1.0;
+  else if (ones) accum[i] = 1.0;
+}
+
+// after the seam donors are in: ghost and NoData cells take no part in the walk, cells without donors are its sources
+__global__ void __launch_bounds__(256) band_mark_sources_props_kernel(const float *__restrict__ props, uint32_t *st, int W,
+                                                                       int H, int y_lo, int y_hi) {
+  const size_t n = (size_t)W * H;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int y = (int)(i / W);
+  if (y < y_lo || y >= y_hi || props[9 * i] == kNoDataGen) st[i] = 0;
+  else if ((st[i] & kDepsMask) == 0) st[i] = kSrcFlag;
+}
+
 }  // namespace
+
+// Flow accumulation methods of the band entry points, numbered as rdb200_dev_fa_method_f32_f64: 0 D8, 1 Tarboton,
+// 2 D4, 3 Holmgren (xparam; Quinn = 1.0), 4 Freeman (xparam).
+enum : int { FA_BAND_D8 = 0, FA_BAND_DINF = 1, FA_BAND_D4 = 2, FA_BAND_HOLMGREN = 3, FA_BAND_FREEMAN = 4 };
+
+void check_fa_method(int method, double xparam) {
+  if (method < FA_BAND_D8 || method > FA_BAND_FREEMAN) fail("flow accumulation: unknown method %d", method);
+  if ((method == FA_BAND_HOLMGREN || method == FA_BAND_FREEMAN) && !std::isfinite(xparam))
+    fail("flow accumulation: method %d needs a finite exponent, got %g", method, xparam);
+}
 
 struct FaccState {
   int W = 0, H = 0, gt = 0, gb = 0;
   bool dinf = false;
+  int method = FA_BAND_D8;
+  bool mfd = false;       // D4 / Holmgren / Freeman: 9-float proportions, accum_levels_kernel<2, true>
   double *accum = nullptr;
   DevBuf<uint8_t> code;
   DevBuf<float> rmax;
+  DevBuf<float> props;
   DevBuf<uint32_t> st;
   DevBuf<int> ghostcnt, fr0, fr1, cnt;
   bool prepared = false;
@@ -2072,15 +2147,19 @@ struct FaccState {
   size_t n() const { return (size_t)W * H; }
 
   void begin(const float *d_dem, double *d_accum, int w, int h, float nodata, int ghost_top, int ghost_bottom,
-             bool dinf_, bool ones) {
+             int method_, double xparam, bool ones) {
     Ctx &c = ctx();
+    check_fa_method(method_, xparam);
     W = w;
     H = h;
     gt = ghost_top ? 1 : 0;
     gb = ghost_bottom ? 1 : 0;
-    dinf = dinf_;
+    method = method_;
+    dinf = method == FA_BAND_DINF;
+    mfd = method >= FA_BAND_D4;
     accum = d_accum;
     if (h - gt - gb < 1) fail("facc_begin: band has no owned rows");
+    if (mfd) return begin_props(d_dem, nodata, xparam, ones);
     packed = !dinf && ones && (w & 3) == 0 && ((uintptr_t)d_accum & 15) == 0 && c.params.accum_packed != 0;
     packed_dinf = dinf && ones && (w & 3) == 0 && ((uintptr_t)d_accum & 15) == 0 && c.params.accum_dinf_packed != 0;
     if (packed_dinf) {
@@ -2124,11 +2203,46 @@ struct FaccState {
     RDB_CK(cudaGetLastError());
   }
 
+  // D4 / Holmgren / Freeman: the proportions of the whole local raster by the single-GPU kernels.  The owned rows see
+  // their full 3 x 3 neighbourhood (the ghost rows hold the neighbours' elevations), so theirs are the single-GPU bits.
+  // Ghost rows are local edge rows: no flow, except that a NoData ghost cell still gets slot 0 == NO_DATA_GEN (every
+  // FM_* cell function tests NoData before the edge), so the walk drops flow into it as on one GPU.  Donor counts of
+  // the owned rows are scattered here; the seam masks (set_ghost_codes) add the neighbours' shares to the edge rows.
+  void begin_props(const float *d_dem, float nodata, double xparam, bool ones) {
+    Ctx &c = ctx();
+    props.alloc(9 * n());
+    st.alloc(n());
+    ghostcnt.alloc(2 * (size_t)W);
+    fr0.alloc(n());
+    fr1.alloc(n());
+    cnt.alloc(4);
+    RDB_CK(cudaMemsetAsync(ghostcnt.p, 0, 2 * (size_t)W * sizeof(int), c.stream));
+    RDB_CK(cudaMemsetAsync(cnt.p, 0, 4 * sizeof(int), c.stream));
+    RDB_CK(cudaMemsetAsync(st.p, 0, n() * sizeof(uint32_t), c.stream));
+    if (method == FA_BAND_D4) fm_d4_dev(d_dem, props.p, W, H, nodata);
+    else if (method == FA_BAND_HOLMGREN) fm_holmgren_dev(d_dem, props.p, W, H, nodata, xparam);
+    else fm_freeman_dev(d_dem, props.p, W, H, nodata, xparam);
+    const unsigned blocks = (unsigned)((n() + 255) / 256);
+    deps_scatter_props_kernel<<<blocks, 256, 0, c.stream>>>(props.p, st.p, W, H);
+    RDB_CK(cudaGetLastError());
+    band_init_props_accum_kernel<<<blocks, 256, 0, c.stream>>>(props.p, accum, W, H, gt, H - gb, ones ? 1 : 0);
+    RDB_CK(cudaGetLastError());
+    count_launch(2);
+  }
+
   int edge_row(int which) const { return which == 0 ? gt : H - 1 - gb; }   // my first / last owned row
   int ghost_row(int which) const { return which == 0 ? 0 : H - 1; }
 
+  // D8 / D-infinity: the flow codes (and rmax) of my edge row; proportions: its seam donor mask (d_rmax_row unused)
   void get_edge_codes(int which, uint8_t *d_code_row, float *d_rmax_row) {
     Ctx &c = ctx();
+    if (mfd) {
+      band_seam_mask_kernel<<<(unsigned)((W + 255) / 256), 256, 0, c.stream>>>(props.p, d_code_row, W, edge_row(which),
+                                                                                which == 0 ? -1 : 1);
+      RDB_CK(cudaGetLastError());
+      count_launch();
+      return;
+    }
     const size_t o = (size_t)edge_row(which) * W;
     RDB_CK(cudaMemcpyAsync(d_code_row, code.p + o, W, cudaMemcpyDeviceToDevice, c.stream));
     if (dinf && d_rmax_row)
@@ -2137,6 +2251,14 @@ struct FaccState {
   void set_ghost_codes(int which, const uint8_t *d_code_row, const float *d_rmax_row) {
     Ctx &c = ctx();
     if ((which == 0 && !gt) || (which == 1 && !gb)) fail("facc_set_ghost_codes: no ghost row on that side");
+    if (mfd) {  // the neighbour's seam donor mask: its shares that flow into my edge row
+      if (prepared) fail("facc_set_ghost_codes: the seam donors must be in before the first run");
+      band_add_seam_donors_kernel<<<(unsigned)((W + 255) / 256), 256, 0, c.stream>>>(d_code_row,
+                                                                                      st.p + (size_t)edge_row(which) * W, W);
+      RDB_CK(cudaGetLastError());
+      count_launch();
+      return;
+    }
     const size_t o = (size_t)ghost_row(which) * W;
     RDB_CK(cudaMemcpyAsync(code.p + o, d_code_row, W, cudaMemcpyDeviceToDevice, c.stream));
     if (dinf && d_rmax_row)
@@ -2246,6 +2368,29 @@ struct FaccState {
     c.stats.accum_rounds = rounds;
   }
 
+  // multi-receiver graphs (D-infinity: MODE 1, proportions: MODE 2): one cooperative launch, levels of the frontier
+  // inside the band (accum_levels_kernel); the first run starts from every source, later ones from the cells the
+  // neighbours' inflow completed (fr0)
+  template <int MODE>
+  void run_levels_band(WalkArgs<double> &a) {
+    Ctx &c = ctx();
+    DevBuf<int> lc(4);
+    RDB_CK(cudaMemsetAsync(lc.p, 0, 4 * sizeof(int), c.stream));
+    int per_sm = 0;
+    RDB_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, accum_levels_kernel<MODE, true>, 256, 0));
+    if (per_sm < 1) per_sm = 1;
+    const int grid = c.num_sms * per_sm;
+    int *q0 = fr0.p, *q1 = fr1.p, *counts = lc.p, *lv = lc.p + 3;
+    int seeded = a.frontier ? 1 : 0;
+    int nc = a.nfrontier, budget = (int)(c.params.accum_budget > 0 ? c.params.accum_budget : 4);
+    if (nc > 0) {
+      void *args[] = {(void *)&a, (void *)&q0, (void *)&q1, (void *)&counts, (void *)&nc, (void *)&budget, (void *)&lv, (void *)&seeded};
+      RDB_CK(cudaLaunchCooperativeKernel((const void *)accum_levels_kernel<MODE, true>, dim3(grid), dim3(256), args, 0,
+                                         c.stream));
+      count_launch();
+    }
+  }
+
   // returns the number of flow parcels parked in the ghost rows by this run: [top, bottom]
   void run(int *sent_top, int *sent_bottom) {
     if (packed) return run_packed(sent_top, sent_bottom);
@@ -2254,6 +2399,7 @@ struct FaccState {
     memset(&a, 0, sizeof(a));
     a.code = code.p;
     a.rmaxArr = rmax.p;
+    a.props = props.p;
     a.accum = accum;
     a.st = st.p;
     a.W = W;
@@ -2264,7 +2410,10 @@ struct FaccState {
     a.next_count = cnt.p + 1;
     if (!prepared) {
       const unsigned blocks = (unsigned)((n() + 255) / 256);
-      deps_gather_kernel<<<blocks, 256, 0, c.stream>>>(code.p, st.p, W, H, gt, H - gb, dinf ? 0 : 1);
+      if (mfd)
+        band_mark_sources_props_kernel<<<blocks, 256, 0, c.stream>>>(props.p, st.p, W, H, gt, H - gb);
+      else
+        deps_gather_kernel<<<blocks, 256, 0, c.stream>>>(code.p, st.p, W, H, gt, H - gb, dinf ? 0 : 1);
       RDB_CK(cudaGetLastError());
       count_launch();
       prepared = true;
@@ -2277,23 +2426,10 @@ struct FaccState {
       a.next_frontier = fr1.p;
     }
     RDB_CK(cudaMemsetAsync(cnt.p, 0, 2 * sizeof(int), c.stream));
-    if (dinf) {
-      // one cooperative launch: levels of the frontier inside the band (accum_levels_kernel)
-      DevBuf<int> lc(4);
-      RDB_CK(cudaMemsetAsync(lc.p, 0, 4 * sizeof(int), c.stream));
-      int per_sm = 0;
-      RDB_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, accum_levels_kernel<1, true>, 256, 0));
-      if (per_sm < 1) per_sm = 1;
-      const int grid = c.num_sms * per_sm;
-      int *q0 = fr0.p, *q1 = fr1.p, *counts = lc.p, *lv = lc.p + 3;
-      int seeded = a.frontier ? 1 : 0;
-      int nc = a.nfrontier, budget = (int)(c.params.accum_budget > 0 ? c.params.accum_budget : 4);
-      if (nc > 0) {
-        void *args[] = {(void *)&a, (void *)&q0, (void *)&q1, (void *)&counts, (void *)&nc, (void *)&budget, (void *)&lv, (void *)&seeded};
-        RDB_CK(cudaLaunchCooperativeKernel((const void *)accum_levels_kernel<1, true>, dim3(grid), dim3(256), args, 0,
-                                           c.stream));
-        count_launch();
-      }
+    if (mfd) {
+      run_levels_band<2>(a);
+    } else if (dinf) {
+      run_levels_band<1>(a);
     } else {
       walk<0>(a);
     }
@@ -2392,18 +2528,20 @@ void FaccState::sum_rows(int *d_sums) {
   RDB_CK(cudaGetLastError());
 }
 
-// Row-band (multi-GPU) FA_D8 / FA_Tarboton driven from C++ over a rdb200_comm: the protocol of FaccState (edge codes to
-// the neighbours once, then rounds of: walk | parked outflow of the two seams in ONE message per neighbour (sums and
-// parcel counts) | neighbours' inflow releases cells of the edge rows | a 1-int all-reduce says whether anyone shipped).
+// Row-band (multi-GPU) flow accumulation driven from C++ over a rdb200_comm, for every method of check_fa_method: the
+// protocol of FaccState (edge codes -- or, for proportions, seam donor masks -- to the neighbours once, then rounds of:
+// walk | parked outflow of the two seams in ONE message per neighbour (sums and parcel counts) | neighbours' inflow
+// releases cells of the edge rows | a 1-int all-reduce says whether anyone shipped).
 void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, int w, int hloc, float nodata, int gt, int gb,
-                  bool dinf, bool ones, int *xrounds) {
+                  int method, double xparam, bool ones, int *xrounds) {
   Ctx &c = ctx();
   const int world = comm_world(comm);
   FaccState A;
-  A.begin(d_dem, d_accum, w, hloc, nodata, gt, gb, dinf, ones);
+  A.begin(d_dem, d_accum, w, hloc, nodata, gt, gb, method, xparam, ones);
   gt = A.gt;
   gb = A.gb;
-  // message layout per side: [w doubles: sums | w ints: parcel counts]; codes: [w floats: rmax | w bytes: codes]
+  // message layout per side: [w doubles: sums | w ints: parcel counts]; codes: [w floats: rmax | w bytes: codes or seam
+  // donor masks] (the float half is unused for proportions)
   const size_t msg = (size_t)w * 12;
   DevBuf<uint8_t> buf(4 * msg);
   uint8_t *su = buf.p, *sd = buf.p + msg, *ru = buf.p + 2 * msg, *rd = buf.p + 3 * msg;
@@ -2497,21 +2635,28 @@ struct rdb200_facc_state {
 
 extern "C" {
 
-int rdb200_dev_facc_begin(rdb200_facc_state **state, const float *d_dem, double *d_accum_inout, int32_t width,
-                          int32_t height, float nodata, int32_t ghost_top, int32_t ghost_bottom, int32_t dinf,
-                          int32_t accum_is_ones) {
+int rdb200_dev_facc_begin_method(rdb200_facc_state **state, const float *d_dem, double *d_accum_inout, int32_t width,
+                                 int32_t height, float nodata, int32_t ghost_top, int32_t ghost_bottom, int32_t method,
+                                 double xparam, int32_t accum_is_ones) {
   FACC_TRY
   rdb::ensure_init();
   if (!state || !d_dem || !d_accum_inout) rdb::fail("facc_begin: null pointer");
   auto *s = new rdb200_facc_state();
   try {
-    s->st.begin(d_dem, d_accum_inout, width, height, nodata, ghost_top, ghost_bottom, dinf != 0, accum_is_ones != 0);
+    s->st.begin(d_dem, d_accum_inout, width, height, nodata, ghost_top, ghost_bottom, method, xparam, accum_is_ones != 0);
   } catch (...) {
     delete s;
     throw;
   }
   *state = s;
   FACC_END
+}
+
+int rdb200_dev_facc_begin(rdb200_facc_state **state, const float *d_dem, double *d_accum_inout, int32_t width,
+                          int32_t height, float nodata, int32_t ghost_top, int32_t ghost_bottom, int32_t dinf,
+                          int32_t accum_is_ones) {
+  return rdb200_dev_facc_begin_method(state, d_dem, d_accum_inout, width, height, nodata, ghost_top, ghost_bottom,
+                                      dinf ? rdb::FA_BAND_DINF : rdb::FA_BAND_D8, 0.0, accum_is_ones);
 }
 
 int rdb200_dev_facc_get_edge_codes(rdb200_facc_state *state, int32_t which, uint8_t *d_code_row, float *d_rmax_row) {

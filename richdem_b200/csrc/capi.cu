@@ -604,7 +604,21 @@ int rdb200_mgpu_fa_f32_f64(const rdb200_comm *comm, const float *d_dem, double *
   if (!d_dem || !d_accum) fail("mgpu_fa: null pointer");
   check_dims(w, rows);
   CallScope cs((int64_t)w * rows);
-  mgpu_fa_band(comm, d_dem, d_accum, w, rows, nodata, gt, gb, dinf != 0, ones != 0, &xr);
+  mgpu_fa_band(comm, d_dem, d_accum, w, rows, nodata, gt, gb, dinf ? 1 : 0, 0.0, ones != 0, &xr);
+  cs.done();
+  if (exchange_rounds) *exchange_rounds = xr;
+  CAPI_END
+}
+
+int rdb200_mgpu_fa_method_f32_f64(const rdb200_comm *comm, const float *d_dem, double *d_accum, int32_t w, int32_t rows,
+                                  float nodata, int32_t gt, int32_t gb, int32_t method, double xparam, int32_t ones,
+                                  int32_t *exchange_rounds) {
+  int xr = 0;
+  CAPI_TRY
+  if (!d_dem || !d_accum) fail("mgpu_fa: null pointer");
+  check_dims(w, rows);
+  CallScope cs((int64_t)w * rows);
+  mgpu_fa_band(comm, d_dem, d_accum, w, rows, nodata, gt, gb, method, xparam, ones != 0, &xr);
   cs.done();
   if (exchange_rounds) *exchange_rounds = xr;
   CAPI_END

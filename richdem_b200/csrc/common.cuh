@@ -161,8 +161,9 @@ int comm_world(const rdb200_comm *c);
 void comm_exchange(const rdb200_comm *c, const void *send_up, void *recv_up, const void *send_dn, void *recv_dn, size_t bytes);
 void comm_allreduce(const rdb200_comm *c, void *buf, size_t count, int op);
 void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, int gt, int gb, int row0, int H, int *xrounds);
+// method: 0 D8, 1 Tarboton, 2 D4, 3 Holmgren (xparam; Quinn = 1.0), 4 Freeman (xparam)
 void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, int w, int hloc, float nodata, int gt, int gb,
-                  bool dinf, bool ones, int *xrounds);
+                  int method, double xparam, bool ones, int *xrounds);
 
 // ---- stage entry points implemented in the .cu files (device pointers, ctx stream) -------
 void fill_depressions_dev(float *d_dem, int w, int h, bool topo4 = false);

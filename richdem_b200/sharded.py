@@ -355,11 +355,42 @@ def _fill_band_protocol(local_dem, g_top, g_bot, solver_cls, group, max_rounds, 
     return out, rounds
 
 
-class CudaBandAccumulator:
-    """librichdem_b200's row-band accumulation entry points (rdb200_dev_facc_*)."""
+def fa_method_id(method: Optional[str], exponent: Optional[float], dinf: bool = False) -> Tuple[int, float]:
+    """(method number of the band entry points, exponent) for a FlowAccumulation method name.  ``method=None`` keeps
+    the ``dinf`` switch: D-infinity if set, else D8.  Names and errors are those of :func:`richdem_b200.FlowAccumulation`."""
+    from . import _D4_METHODS, _D8_METHODS, _DINF_METHODS, _EXPONENT_METHODS, _OUT_OF_SCOPE_METHODS
+    if method is None:
+        return (1 if dinf else 0), 0.0
+    if dinf and method not in _DINF_METHODS:
+        raise ValueError(f'dinf=True contradicts method "{method}"')
+    if method in _D8_METHODS:
+        return 0, 0.0
+    if method in _DINF_METHODS:
+        return 1, 0.0
+    if method in _D4_METHODS:
+        return 2, 0.0
+    if method == "Quinn":
+        return 3, 1.0
+    if method in _EXPONENT_METHODS:
+        if exponent is None:
+            raise Exception(f'FlowAccumulation method "{method}" requires an exponent!')
+        return (3 if method == "Holmgren" else 4), float(exponent)
+    if method in _OUT_OF_SCOPE_METHODS:
+        raise Exception(f'FlowAccumulation method "{method}" is outside the GPU hot path '
+                        "(random-walk metric; use the reference CPU implementation)")
+    raise Exception("Invalid FlowAccumulation method. Valid methods are: " +
+                    ", ".join(_DINF_METHODS + ("Quinn",) + _D8_METHODS + _D4_METHODS + _EXPONENT_METHODS +
+                              _OUT_OF_SCOPE_METHODS))
 
-    def __init__(self, local_dem, local_accum, nodata: float, g_top: int, g_bot: int, dinf: bool, ones: bool):
+
+class CudaBandAccumulator:
+    """librichdem_b200's row-band accumulation entry points (rdb200_dev_facc_*).  ``method`` / ``exponent`` as in
+    :func:`richdem_b200.FlowAccumulation`; without a method, ``dinf`` picks D-infinity or D8."""
+
+    def __init__(self, local_dem, local_accum, nodata: float, g_top: int, g_bot: int, dinf: bool, ones: bool,
+                 method: Optional[str] = None, exponent: Optional[float] = None):
         from . import _lib
+        mid, xparam = fa_method_id(method, exponent, dinf)
         assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
         assert _on_device(local_accum) and local_accum.dtype == torch.float64 and local_accum.is_contiguous()
         self._lib = _lib
@@ -367,12 +398,12 @@ class CudaBandAccumulator:
         self.L = _lib.lib()
         self.h, self.w = local_dem.shape
         self.dev = local_dem.device
-        self.dinf = dinf
+        self.dinf = mid == 1
         self._dem, self._accum = local_dem, local_accum  # the library reads the elevations again at the first run
         self._state = C.c_void_p()
-        _lib.check(self.L.rdb200_dev_facc_begin(C.byref(self._state), local_dem.data_ptr(), local_accum.data_ptr(),
-                                                self.w, self.h, float(nodata), int(g_top), int(g_bot), int(dinf),
-                                                int(ones)))
+        _lib.check(self.L.rdb200_dev_facc_begin_method(C.byref(self._state), local_dem.data_ptr(), local_accum.data_ptr(),
+                                                       self.w, self.h, float(nodata), int(g_top), int(g_bot), mid,
+                                                       xparam, int(ones)))
 
     def edge_codes(self, which: int):
         code = torch.empty(self.w, dtype=torch.uint8, device=self.dev)
@@ -404,13 +435,17 @@ class CudaBandAccumulator:
 
 def fa_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: float, dinf: bool = False,
             weights: Optional["torch.Tensor"] = None, rank_rows=None, group=None, max_rounds: int = 1000000,
-            return_stats: bool = False, accumulator_cls=None):
-    """FA_D8 / FA_Tarboton over this rank's band.  ``local_dem`` is (g_top + owned + g_bot) x W and
+            return_stats: bool = False, accumulator_cls=None, method: Optional[str] = None,
+            exponent: Optional[float] = None):
+    """FlowAccumulation over this rank's band.  ``local_dem`` is (g_top + owned + g_bot) x W and
     its ghost rows must already hold the neighbouring bands' elevations (``fill_band`` leaves them so;
     otherwise call :func:`exchange_rows`).  ``weights`` (float64, same local shape) defaults to ones.
+    ``method`` / ``exponent`` as in :func:`richdem_b200.FlowAccumulation` (D8, Dinf, D4, Quinn, Holmgren, Freeman and
+    their aliases); without a method, ``dinf`` picks FA_Tarboton or FA_D8.
     Returns (local accumulation incl. scratch ghost rows, exchange rounds[, stats])."""
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     world = dist.get_world_size(group) if dist.is_initialized() else 1
+    mid, xparam = fa_method_id(method, exponent, dinf)
     import os
     if accumulator_cls is None and os.environ.get("RDB_BAND_DRIVER", "cxx") != "python":
         from . import _lib
@@ -421,16 +456,16 @@ def fa_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: float, di
         _lib.use_torch_stream()
         xr = C.c_int32(0)
         cm = lib_comm(group)
-        _lib.check(_lib.lib().rdb200_mgpu_fa_f32_f64(cm.handle, local_dem.data_ptr(), acc.data_ptr(), local_dem.shape[1],
-                                                     local_dem.shape[0], float(nodata), int(g_top), int(g_bot), int(dinf),
-                                                     int(ones), C.byref(xr)))
+        _lib.check(_lib.lib().rdb200_mgpu_fa_method_f32_f64(cm.handle, local_dem.data_ptr(), acc.data_ptr(), local_dem.shape[1],
+                                                            local_dem.shape[0], float(nodata), int(g_top), int(g_bot), mid,
+                                                            xparam, int(ones), C.byref(xr)))
         if return_stats:
             return acc, int(xr.value), _lib.stats()
         return acc, int(xr.value)
     accumulator_cls = accumulator_cls or CudaBandAccumulator
     ones = weights is None
     acc = torch.empty(local_dem.shape, dtype=torch.float64, device=local_dem.device) if ones else weights
-    A = accumulator_cls(local_dem, acc, nodata, g_top, g_bot, dinf, ones)
+    A = accumulator_cls(local_dem, acc, nodata, g_top, g_bot, dinf, ones, method=method, exponent=exponent)
     if world > 1:
         up = A.edge_codes(0) if g_top else None
         dn = A.edge_codes(1) if g_bot else None
