@@ -250,6 +250,7 @@ RDB200_API int rdb200_dev_generate_fbm_f32(float *d_dem, int32_t width, int32_t 
  *   rank 0:  rdb200_nccl_unique_id(id)   ... ship the 128 bytes to every rank (MPI_Bcast, a file, torch.distributed) ...
  *   all:     rdb200_init(local_gpu); rdb200_comm_create_nccl(&comm, rank, world, id);
  *            rdb200_mgpu_fill_depressions_d8_f32(comm, d_band, W, rows, gt, gb, row0, H, NULL);
+ *            rdb200_mgpu_resolve_flats_epsilon_f32(comm, d_band, W, rows, nodata, gt, gb, NULL);
  *            rdb200_mgpu_fa_f32_f64(comm, d_band, d_accum, W, rows, nodata, gt, gb, 0, 1, NULL);
  */
 typedef struct rdb200_comm rdb200_comm;
@@ -273,6 +274,15 @@ RDB200_API int rdb200_comm_destroy(rdb200_comm *comm);
 RDB200_API int rdb200_mgpu_fill_depressions_d8_f32(const rdb200_comm *comm, float *d_band, int32_t width, int32_t local_rows,
                                                    int32_t ghost_top, int32_t ghost_bottom, int32_t row0, int32_t height,
                                                    int32_t *exchange_rounds);
+/* ResolveFlatsEpsilon (include/richdem/flats/flats.hpp:21-28) over row bands, in place on the owned rows of `d_band`
+ * (local_rows x width; the ghost rows must hold the neighbours' edge rows on entry, as the fill leaves them, and hold
+ * the neighbours' resolved edge rows on return, ready for rdb200_mgpu_fa_*).  Same result as the single-GPU call, bit for
+ * bit.  comm and d_band must not be null; ghost_top / ghost_bottom must be exactly (rank > 0) / (rank < world - 1) and
+ * the band must own at least one row -- these are checked before any communication.  *seam_iterations (optional): rounds
+ * of the outlet-flag and flat-height merges across seams (0 for one band). */
+RDB200_API int rdb200_mgpu_resolve_flats_epsilon_f32(const rdb200_comm *comm, float *d_band, int32_t width, int32_t local_rows,
+                                                     float nodata, int32_t ghost_top, int32_t ghost_bottom,
+                                                     int32_t *seam_iterations);
 /* FA_D8 (dinf = 0) / FA_Tarboton (dinf = 1) (include/richdem/methods/flow_accumulation.hpp:27,16) over row bands.
  * d_band_dem: elevations incl. ghost rows (neighbours' rows); d_band_accum_inout: weights in / accumulation out on the
  * owned rows (the ghost rows are scratch); accum_is_ones as in rdb200_fa_d8_f32_f64. */
@@ -372,8 +382,8 @@ RDB200_API int rdb200_dev_facc_finish(rdb200_facc_state *state);
 /* Same role as ResolveFlatsEpsilon (include/richdem/flats/flats.hpp:21-28) for one row band; the
  * local elevation raster (ghost_top + owned + ghost_bottom rows, ghost rows = the neighbours' rows)
  * is modified in place on the owned rows.  The steps run the single-GPU kernels on the local
- * raster; between them the caller moves the seam rows (see the protocol in csrc/flats.cu and
- * richdem_b200/sharded.py: resolve_flats_band). */
+ * raster; between them the caller moves the seam rows (see the protocol in csrc/flats.cu, which
+ * rdb200_mgpu_resolve_flats_epsilon_f32 runs in one collective call). */
 typedef struct rdb200_flats_state rdb200_flats_state;
 RDB200_API int rdb200_dev_flats_begin(rdb200_flats_state **state, float *d_dem, int32_t width, int32_t height,
                                       float nodata, int32_t ghost_top, int32_t ghost_bottom);

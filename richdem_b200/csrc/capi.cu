@@ -624,4 +624,17 @@ int rdb200_mgpu_fa_method_f32_f64(const rdb200_comm *comm, const float *d_dem, d
   CAPI_END
 }
 
+int rdb200_mgpu_resolve_flats_epsilon_f32(const rdb200_comm *comm, float *d_band, int32_t w, int32_t rows, float nodata,
+                                          int32_t gt, int32_t gb, int32_t *seam_iterations) {
+  int it = 0;
+  CAPI_TRY
+  if (!comm || !d_band) fail("mgpu_resolve_flats: null pointer");
+  check_dims(w, rows);
+  CallScope cs((int64_t)w * rows);
+  mgpu_resolve_flats_band(comm, d_band, w, rows, nodata, gt, gb, &it);
+  cs.done();
+  if (seam_iterations) *seam_iterations = it;
+  CAPI_END
+}
+
 }  // extern "C"

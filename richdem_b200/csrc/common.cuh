@@ -164,6 +164,10 @@ void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, in
 // method: 0 D8, 1 Tarboton, 2 D4, 3 Holmgren (xparam; Quinn = 1.0), 4 Freeman (xparam)
 void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, int w, int hloc, float nodata, int gt, int gb,
                   int method, double xparam, bool ones, int *xrounds);
+void mgpu_resolve_flats_band(const rdb200_comm *comm, float *d_local, int w, int hloc, float nodata, int gt, int gb,
+                             int *seam_iters);
+// the band relaxation protocol over a state that holds its start; R sweep rounds between halo exchanges (0: none)
+int mgpu_relax_band(const rdb200_comm *comm, rdb200_fill_state *state, int gt, int gb, int R);
 
 // ---- stage entry points implemented in the .cu files (device pointers, ctx stream) -------
 void fill_depressions_dev(float *d_dem, int w, int h, bool topo4 = false);

@@ -1599,6 +1599,41 @@ void finish_band_distance_state(rdb200_fill_state *s, float *d_out) {
   RDB_CK(cudaStreamSynchronize(ctx().stream));
   delete s;
 }
+
+// The band relaxation of mgpu_fill_band without its multigrid start and coarse corrections, for a state that already
+// holds its start (the flat-resolution gradients' distance states): cycles of R sweep rounds (0: to the band's local
+// fixed point) | edge rows to the neighbours, ghost rows drop to them where lower | one 2-int MAX all-reduce of {tiles
+// still active, a ghost row dropped}.  Every value is a decreasing upper bound, so when neither happened on any rank
+// the bands hold the single-GPU fixed point.  Returns the number of cycles.
+int mgpu_relax_band(const rdb200_comm *comm, rdb200_fill_state *state, int gt, int gb, int R) {
+  Ctx &c = ctx();
+  FillState &st = state->st;
+  const int world = comm_world(comm), w = st.W, h = st.H;
+  DevBuf<float> rows(4 * (size_t)w);  // send up, send down, receive up, receive down
+  DevBuf<int> flags(2);               // tiles active | a ghost row dropped
+  float *send_up = rows.p, *send_dn = rows.p + w, *recv_up = rows.p + 2 * (size_t)w, *recv_dn = rows.p + 3 * (size_t)w;
+  int *hflags = (int *)c.pinned + 1024;  // (FillState::run reads its control block back into the front of the scratch)
+  for (int cycles = 1;; cycles++) {
+    if (cycles > 100000) fail("mgpu_relax_band: no convergence");
+    const bool active = (st.run(world > 1 ? R : 0) & 4) != 0;
+    if (world == 1) {
+      if (active) continue;
+      RDB_CK(cudaStreamSynchronize(c.stream));
+      return cycles;
+    }
+    RDB_CK(cudaMemsetAsync(flags.p, 0, 2 * sizeof(int), c.stream));
+    if (gt) st.read_row(1, send_up);
+    if (gb) st.read_row(h - 2, send_dn);
+    comm_exchange(comm, send_up, recv_up, send_dn, recv_dn, (size_t)w * sizeof(float));
+    if (gt) st.ghost_update(0, recv_up, flags.p + 1);
+    if (gb) st.ghost_update(h - 1, recv_dn, flags.p + 1);
+    if (active) fill_i32_kernel<<<1, 1, 0, c.stream>>>(flags.p, 1, 1);
+    comm_allreduce(comm, flags.p, 2, RDB200_MAX_I32);
+    RDB_CK(cudaMemcpyAsync(hflags, flags.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+    RDB_CK(cudaStreamSynchronize(c.stream));
+    if (!(hflags[0] | hflags[1])) return cycles;
+  }
+}
 }  // namespace rdb
 
 namespace rdb {

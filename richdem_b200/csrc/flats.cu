@@ -22,6 +22,7 @@
 #include <algorithm>
 #include <chrono>
 #include <cstdlib>
+#include <memory>
 
 #include <cooperative_groups.h>
 namespace cg = cooperative_groups;
@@ -865,13 +866,14 @@ void d8_flow_directions_flats_dev(float *d_dem, uint8_t *d_dirs, int w, int h, f
 // =================================================================================================
 // Row-band (multi-GPU) flat resolution.  The stencil / union-find / seeding / conversion / apply
 // kernels above run unchanged on the local raster (ghost_top + owned + ghost_bottom rows); what
-// crosses a seam is moved by the caller (richdem_b200/sharded.py) between the steps below:
+// crosses a seam moves between the steps below (mgpu_resolve_flats_band drives them over a
+// rdb200_comm; the rdb200_dev_flats_* entry points expose them one by one):
 //   begin (classify)            -> exchange flag rows (IS_A_FLAT / NoData of the ghost rows)
 //   edges                       -> exchange flag rows again (low / high edge bits)
 //   components (local union-find over owned + ghost rows, outlet flag per local root)
 //                               -> OR the outlet flags of roots that meet at a seam until stable
 //   labels
-//   gradient_begin(away)        -> band distance protocol (rdb200_dev_fill_run / read_row / update_row)
+//   gradient_begin(away)        -> band distance protocol (mgpu_relax_band)
 //   gradient_end(away)          -> MAX the flat heights of roots that meet at a seam until stable
 //   gradient_begin/end(towards) -> band distance protocol
 //   apply, finish
@@ -889,26 +891,60 @@ struct rdb200_flats_state {
 
 namespace rdb {
 void capi_set_error(const char *msg);
+
+namespace {
+
+// ---- seam messages: a side's message is [my edge row | my ghost row] (2 x W entries).  The neighbour's edge row is my
+// ghost row and its ghost row is my edge row, so entry [0][x] of what arrives belongs to my ghost cell x and [1][x] to
+// my edge cell x.  Rows are local row numbers (edge, ghost) of the side.
+
+// outlet flag of the component (local union-find root) of every seam cell
+__global__ void __launch_bounds__(256) seam_flag_payload_kernel(const int *__restrict__ root, const uint8_t *__restrict__ rootflag,
+                                                                 int W, int edge, int ghost, uint8_t *__restrict__ msg) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= W) return;
+  const int y = blockIdx.y == 0 ? edge : ghost;
+  msg[(size_t)blockIdx.y * W + x] = rootflag[root[(size_t)y * W + x]];
 }
 
-#define FLATS_TRY try {
-#define FLATS_END                      \
-  }                                    \
-  catch (const std::exception &e) {    \
-    rdb::capi_set_error(e.what());     \
-    return 1;                          \
-  }                                    \
-  return 0;
+// a flag the neighbour has for a data cell sets the flag of my component of that cell; *changed = 1 if one went 0 -> 1
+// (every writer stores 1: a plain byte store)
+__global__ void __launch_bounds__(256) seam_merge_flags_kernel(const uint8_t *__restrict__ ft, const int *__restrict__ root,
+                                                                uint8_t *rootflag, int W, int edge, int ghost,
+                                                                const uint8_t *__restrict__ theirs, int *changed) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= W) return;
+  const size_t i = (size_t)(blockIdx.y == 0 ? ghost : edge) * W + x;
+  if (!theirs[(size_t)blockIdx.y * W + x] || (ft[i] & FT_NODATA)) return;
+  const int r = root[i];
+  if (!rootflag[r]) {
+    rootflag[r] = 1;
+    *changed = 1;
+  }
+}
 
-extern "C" {
+// flat height (deepest away level) of the flat of every seam cell, 0 for cells outside a drainable flat
+__global__ void __launch_bounds__(256) seam_height_payload_kernel(const int *__restrict__ labels, const int *__restrict__ Hh, int W,
+                                                                   int edge, int ghost, int *__restrict__ msg) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= W) return;
+  const int lab = labels[(size_t)(blockIdx.y == 0 ? edge : ghost) * W + x];
+  msg[(size_t)blockIdx.y * W + x] = lab > 0 ? Hh[lab - 1] : 0;
+}
 
-int rdb200_dev_flats_begin(rdb200_flats_state **state, float *d_dem, int32_t width, int32_t height, float nodata,
-                           int32_t ghost_top, int32_t ghost_bottom) {
-  FLATS_TRY
-  using namespace rdb;
-  ensure_init();
-  if (!state || !d_dem) fail("flats_begin: null pointer");
-  if (height - (ghost_top ? 1 : 0) - (ghost_bottom ? 1 : 0) < 1) fail("flats_begin: band has no owned rows");
+// the neighbour's flat heights MAX into mine; *changed = 1 if one grew
+__global__ void __launch_bounds__(256) seam_merge_heights_kernel(const int *__restrict__ labels, int *Hh, int W, int edge, int ghost,
+                                                                  const int *__restrict__ theirs, int *changed) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= W) return;
+  const int lab = labels[(size_t)(blockIdx.y == 0 ? ghost : edge) * W + x];
+  if (lab <= 0) return;
+  const int v = theirs[(size_t)blockIdx.y * W + x];
+  if (v > Hh[lab - 1] && atomicMax(&Hh[lab - 1], v) < v) *changed = 1;  // (heights only grow: a stale read only lets more through)
+}
+
+// ---- the steps (shared by the C++ band driver and the step-wise entry points) ----
+rdb200_flats_state *flats_begin(float *d_dem, int width, int height, float nodata, int ghost_top, int ghost_bottom) {
   Ctx &c = ctx();
   auto *s = new rdb200_flats_state();
   try {
@@ -938,7 +974,177 @@ int rdb200_dev_flats_begin(rdb200_flats_state **state, float *d_dem, int32_t wid
     delete s;
     throw;
   }
-  *state = s;
+  return s;
+}
+
+void flats_edges(rdb200_flats_state *s) {
+  Ctx &c = ctx();
+  flats_edges_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->dem, s->ft.p, s->W, s->H, s->dev.p);
+  RDB_CK(cudaGetLastError());
+  RDB_CK(cudaStreamSynchronize(c.stream));
+}
+
+void flats_components(rdb200_flats_state *s) {
+  Ctx &c = ctx();
+  uf_build(s->dem, s->ft.p, s->parent.p, s->W, s->H);
+  uf_roots_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->ft.p, s->parent.p, s->labels.p, s->rootflag.p, s->n());
+  RDB_CK(cudaGetLastError());
+  RDB_CK(cudaStreamSynchronize(c.stream));
+}
+
+void flats_labels(rdb200_flats_state *s) {
+  Ctx &c = ctx();
+  make_labels_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->rootflag.p, s->ft.p, s->labels.p, s->n());
+  RDB_CK(cudaGetLastError());
+  RDB_CK(cudaStreamSynchronize(c.stream));
+}
+
+rdb200_fill_state *flats_gradient_begin(rdb200_flats_state *s, bool away) {
+  Ctx &c = ctx();
+  int *dist = away ? s->away.p : s->tw.p;
+  gradient_seed_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->dem, s->ft.p, s->labels.p, reinterpret_cast<float *>(dist), s->W, s->H,
+                                                          away ? 1 : 0);
+  RDB_CK(cudaGetLastError());
+  return new_band_distance_state(s->ft.p, FT_FLAT, reinterpret_cast<const float *>(dist), s->W, s->H, s->gt, s->gb);
+}
+
+void flats_gradient_end(rdb200_flats_state *s, bool away, rdb200_fill_state *dist_state) {
+  Ctx &c = ctx();
+  int *dist = away ? s->away.p : s->tw.p;
+  finish_band_distance_state(dist_state, reinterpret_cast<float *>(dist));
+  gradient_convert_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->ft.p, s->labels.p, dist, s->Hh.p, s->n(), away ? 1 : 0, s->dev.p);
+  RDB_CK(cudaGetLastError());
+  RDB_CK(cudaStreamSynchronize(c.stream));
+}
+
+void flats_apply(rdb200_flats_state *s) {
+  Ctx &c = ctx();
+  flats_apply_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->dem, s->labels.p, s->away.p, s->tw.p, s->Hh.p, nullptr, nullptr, s->W,
+                                                        s->H, 1, s->dev.p);
+  RDB_CK(cudaGetLastError());
+  FlatDev *hd = (FlatDev *)c.pinned;
+  RDB_CK(cudaMemcpyAsync(hd, s->dev.p, sizeof(FlatDev), cudaMemcpyDeviceToHost, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  if (hd->dist_overflow) fail("resolve_flats (band): a flat is more than 2^24 cells long; float distances are not exact there");
+}
+
+}  // namespace
+
+// ResolveFlatsEpsilon over row bands, driven from C++ over a rdb200_comm: the protocol above, in that order.  Flag rows
+// go straight from the flag array into the neighbours' ghost rows; the seam merges are the kernels above, and a merge
+// loop ends when a 1-int MAX all-reduce says that no rank's merge changed anything.  The two gradients are band
+// relaxations (mgpu_relax_band) of the distance states, with R = 64 sweep rounds between halo exchanges when there are
+// several bands.  On return the ghost rows of d_local hold the neighbours' resolved edge rows (one last exchange), so
+// that accumulation can follow without another one.  *seam_iters: flag + height merge iterations (0 for one band).
+void mgpu_resolve_flats_band(const rdb200_comm *comm, float *d_local, int w, int hloc, float nodata, int gt, int gb,
+                             int *seam_iters) {
+  Ctx &c = ctx();
+  const int rank = comm_rank(comm), world = comm_world(comm);
+  // every check comes before the first collective: a rank that fails here must not leave its peers waiting
+  if (!comm || !d_local) fail("mgpu_resolve_flats: null pointer");
+  if (w < 1 || hloc - (gt ? 1 : 0) - (gb ? 1 : 0) < 1) fail("mgpu_resolve_flats: band has no owned rows (%d x %d)", w, hloc);
+  if ((gt != 0) != (rank > 0) || (gb != 0) != (rank < world - 1))
+    fail("mgpu_resolve_flats: rank %d of %d needs ghost_top = %d and ghost_bottom = %d (got %d, %d)", rank, world, rank > 0 ? 1 : 0,
+         rank < world - 1 ? 1 : 0, gt, gb);
+  gt = gt ? 1 : 0;
+  gb = gb ? 1 : 0;
+  std::unique_ptr<rdb200_flats_state> s(flats_begin(d_local, w, hloc, nodata, gt, gb));
+  const int edge[2] = {gt, hloc - 1 - gb}, ghost[2] = {0, hloc - 1};  // per side: 0 = top, 1 = bottom
+  const bool side_on[2] = {gt != 0, gb != 0};
+  // one edge row of `p` (elem bytes per cell) to each neighbour's ghost row, in place
+  auto exchange_rows = [&](void *p, size_t elem) {
+    uint8_t *b = static_cast<uint8_t *>(p);
+    const size_t row = (size_t)w * elem;
+    comm_exchange(comm, b + edge[0] * row, b + ghost[0] * row, b + edge[1] * row, b + ghost[1] * row, row);
+  };
+  // message buffers: send up, send down, receive up, receive down; 2 rows of int32 at most
+  const size_t msg = (size_t)w * 2 * sizeof(int);
+  DevBuf<uint8_t> buf(4 * msg);
+  uint8_t *snd[2] = {buf.p, buf.p + msg}, *rcv[2] = {buf.p + 2 * msg, buf.p + 3 * msg};
+  DevBuf<int> changed(1);
+  int *hchanged = (int *)c.pinned + 1024;
+  const dim3 blk(256), grd((unsigned)((w + 255) / 256), 2);
+  // merge rounds until no rank changed anything; returns the number of rounds
+  auto merge_until_stable = [&](bool heights) {
+    int it = 0;
+    while (world > 1) {
+      if (++it > 1000000) fail("mgpu_resolve_flats: seam merges do not settle");
+      RDB_CK(cudaMemsetAsync(changed.p, 0, sizeof(int), c.stream));
+      for (int k = 0; k < 2; k++) {
+        if (!side_on[k]) continue;
+        if (heights)
+          seam_height_payload_kernel<<<grd, blk, 0, c.stream>>>(s->labels.p, s->Hh.p, w, edge[k], ghost[k],
+                                                                reinterpret_cast<int *>(snd[k]));
+        else
+          seam_flag_payload_kernel<<<grd, blk, 0, c.stream>>>(s->labels.p, s->rootflag.p, w, edge[k], ghost[k], snd[k]);
+      }
+      RDB_CK(cudaGetLastError());
+      comm_exchange(comm, snd[0], rcv[0], snd[1], rcv[1], heights ? msg : (size_t)w * 2);
+      for (int k = 0; k < 2; k++) {
+        if (!side_on[k]) continue;
+        if (heights)
+          seam_merge_heights_kernel<<<grd, blk, 0, c.stream>>>(s->labels.p, s->Hh.p, w, edge[k], ghost[k],
+                                                               reinterpret_cast<const int *>(rcv[k]), changed.p);
+        else
+          seam_merge_flags_kernel<<<grd, blk, 0, c.stream>>>(s->ft.p, s->labels.p, s->rootflag.p, w, edge[k], ghost[k], rcv[k],
+                                                             changed.p);
+      }
+      RDB_CK(cudaGetLastError());
+      count_launch(2 * (gt + gb));
+      comm_allreduce(comm, changed.p, 1, RDB200_MAX_I32);
+      RDB_CK(cudaMemcpyAsync(hchanged, changed.p, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+      RDB_CK(cudaStreamSynchronize(c.stream));
+      if (*hchanged == 0) break;
+    }
+    return it;
+  };
+  const int R = world > 1 ? 64 : 0;  // sweep rounds between halo exchanges (0: one band relaxes to its fixed point)
+
+  exchange_rows(s->ft.p, 1);  // IS_A_FLAT / NoData of the ghost rows
+  flats_edges(s.get());
+  exchange_rows(s->ft.p, 1);  // low / high edge bits of the ghost rows
+  flats_components(s.get());
+  int iters = merge_until_stable(false);  // (labels holds every cell's root until flats_labels)
+  flats_labels(s.get());
+  for (const bool away : {true, false}) {
+    rdb200_fill_state *ds = flats_gradient_begin(s.get(), away);
+    try {
+      mgpu_relax_band(comm, ds, gt, gb, R);
+    } catch (...) {
+      rdb200_dev_fill_finish(ds, nullptr);
+      throw;
+    }
+    flats_gradient_end(s.get(), away, ds);
+    if (away) iters += merge_until_stable(true);
+  }
+  flats_apply(s.get());
+  s.reset();
+  exchange_rows(d_local, sizeof(float));  // the neighbours' resolved edge rows
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  if (seam_iters) *seam_iters = iters;
+}
+
+}  // namespace rdb
+
+#define FLATS_TRY try {
+#define FLATS_END                      \
+  }                                    \
+  catch (const std::exception &e) {    \
+    rdb::capi_set_error(e.what());     \
+    return 1;                          \
+  }                                    \
+  return 0;
+
+extern "C" {
+
+int rdb200_dev_flats_begin(rdb200_flats_state **state, float *d_dem, int32_t width, int32_t height, float nodata,
+                           int32_t ghost_top, int32_t ghost_bottom) {
+  FLATS_TRY
+  using namespace rdb;
+  ensure_init();
+  if (!state || !d_dem) fail("flats_begin: null pointer");
+  if (height - (ghost_top ? 1 : 0) - (ghost_bottom ? 1 : 0) < 1) fail("flats_begin: band has no owned rows");
+  *state = flats_begin(d_dem, width, height, nodata, ghost_top, ghost_bottom);
   FLATS_END
 }
 
@@ -961,72 +1167,38 @@ int rdb200_dev_flats_arrays(rdb200_flats_state *s, uint64_t *out6) {
 
 int rdb200_dev_flats_edges(rdb200_flats_state *s) {
   FLATS_TRY
-  using namespace rdb;
-  Ctx &c = ctx();
-  flats_edges_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->dem, s->ft.p, s->W, s->H, s->dev.p);
-  RDB_CK(cudaGetLastError());
-  RDB_CK(cudaStreamSynchronize(c.stream));
+  rdb::flats_edges(s);
   FLATS_END
 }
 
 int rdb200_dev_flats_components(rdb200_flats_state *s) {
   FLATS_TRY
-  using namespace rdb;
-  Ctx &c = ctx();
-  const size_t n = s->n();
-  uf_build(s->dem, s->ft.p, s->parent.p, s->W, s->H);
-  uf_roots_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->ft.p, s->parent.p, s->labels.p, s->rootflag.p, n);
-  RDB_CK(cudaGetLastError());
-  RDB_CK(cudaStreamSynchronize(c.stream));
+  rdb::flats_components(s);
   FLATS_END
 }
 
 int rdb200_dev_flats_labels(rdb200_flats_state *s) {
   FLATS_TRY
-  using namespace rdb;
-  Ctx &c = ctx();
-  make_labels_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->rootflag.p, s->ft.p, s->labels.p, s->n());
-  RDB_CK(cudaGetLastError());
-  RDB_CK(cudaStreamSynchronize(c.stream));
+  rdb::flats_labels(s);
   FLATS_END
 }
 
 int rdb200_dev_flats_gradient_begin(rdb200_flats_state *s, int32_t away, rdb200_fill_state **dist_state) {
   FLATS_TRY
-  using namespace rdb;
-  Ctx &c = ctx();
-  if (!dist_state) fail("flats_gradient_begin: null pointer");
-  int *dist = away ? s->away.p : s->tw.p;
-  gradient_seed_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->dem, s->ft.p, s->labels.p, reinterpret_cast<float *>(dist),
-                                                          s->W, s->H, away ? 1 : 0);
-  RDB_CK(cudaGetLastError());
-  *dist_state = new_band_distance_state(s->ft.p, FT_FLAT, reinterpret_cast<const float *>(dist), s->W, s->H, s->gt, s->gb);
+  if (!dist_state) rdb::fail("flats_gradient_begin: null pointer");
+  *dist_state = rdb::flats_gradient_begin(s, away != 0);
   FLATS_END
 }
 
 int rdb200_dev_flats_gradient_end(rdb200_flats_state *s, int32_t away, rdb200_fill_state *dist_state) {
   FLATS_TRY
-  using namespace rdb;
-  Ctx &c = ctx();
-  int *dist = away ? s->away.p : s->tw.p;
-  finish_band_distance_state(dist_state, reinterpret_cast<float *>(dist));
-  gradient_convert_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->ft.p, s->labels.p, dist, s->Hh.p, s->n(), away ? 1 : 0, s->dev.p);
-  RDB_CK(cudaGetLastError());
-  RDB_CK(cudaStreamSynchronize(c.stream));
+  rdb::flats_gradient_end(s, away != 0, dist_state);
   FLATS_END
 }
 
 int rdb200_dev_flats_apply(rdb200_flats_state *s) {
   FLATS_TRY
-  using namespace rdb;
-  Ctx &c = ctx();
-  flats_apply_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->dem, s->labels.p, s->away.p, s->tw.p, s->Hh.p, nullptr, nullptr,
-                                                        s->W, s->H, 1, s->dev.p);
-  RDB_CK(cudaGetLastError());
-  FlatDev *hd = (FlatDev *)c.pinned;
-  RDB_CK(cudaMemcpyAsync(hd, s->dev.p, sizeof(FlatDev), cudaMemcpyDeviceToHost, c.stream));
-  RDB_CK(cudaStreamSynchronize(c.stream));
-  if (hd->dist_overflow) fail("resolve_flats (band): a flat is more than 2^24 cells long; float distances are not exact there");
+  rdb::flats_apply(s);
   FLATS_END
 }
 

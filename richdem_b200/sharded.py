@@ -123,16 +123,19 @@ _COMMS = {}
 
 class LibComm:
     """A rdb200_comm for a torch.distributed process group.  NCCL groups get the library's own NCCL communicator (the
-    128-byte unique id travels over torch.distributed once); any other backend (gloo in the CPU tests, where "device"
-    memory is host memory) gets the callback communicator, whose two callbacks move host buffers with torch.distributed."""
+    128-byte unique id travels over torch.distributed once); any other backend gets the callback communicator, whose two
+    callbacks move the messages with torch.distributed.  ``cuda``: the bands live in CUDA memory, so the callbacks stage
+    every message through host tensors (gloo moves host memory); otherwise (the CPU tests, where "device" memory is host
+    memory) they send the buffers in place."""
 
-    def __init__(self, group=None):
+    def __init__(self, group=None, cuda: bool = False):
         from . import _lib
         self._lib = _lib
         L = _lib.lib()
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.group = group
+        self.cuda = bool(cuda)
         self.handle = C.c_void_p()
         backend = dist.get_backend(group) if dist.is_initialized() else "none"
         if backend == "nccl":
@@ -156,16 +159,40 @@ class LibComm:
         buf = (C.c_uint8 * nbytes).from_address(ptr)
         return torch.frombuffer(buf, dtype=dtype)
 
+    def _device(self, ptr, nbytes):
+        return _view(ptr, (nbytes,), "|u1", torch.device("cuda", torch.cuda.current_device()))
+
+    def _to_host(self, ptr, nbytes, dtype):
+        """Host tensor that holds the message at ``ptr`` (a copy for a CUDA band; the library's stream is synchronised
+        before a callback runs, so the copy sees its data)."""
+        if self.cuda:
+            return self._device(ptr, nbytes).cpu().view(dtype)
+        return self._host(ptr, nbytes, dtype)
+
+    def _from_host(self, ptr, host):
+        """Put a host tensor received for ``ptr`` in place (a no-op for host memory: it was received there)."""
+        if self.cuda:
+            self._device(ptr, host.numel() * host.element_size()).copy_(host.view(torch.uint8))
+
+    def _settle(self):
+        if self.cuda:  # the callback returns when the data has arrived
+            torch.cuda.current_stream().synchronize()
+
     def _exchange(self, user, su, ru, sd, rd, nbytes):
         try:
-            ops = []
+            ops, recvs = [], []
             for s_, r_, peer in ((su, ru, self.rank - 1), (sd, rd, self.rank + 1)):
                 if s_:
-                    ops += [dist.P2POp(dist.isend, self._host(s_, nbytes, torch.uint8), peer, self.group),
-                            dist.P2POp(dist.irecv, self._host(r_, nbytes, torch.uint8), peer, self.group)]
+                    recv = torch.empty(nbytes, dtype=torch.uint8) if self.cuda else self._host(r_, nbytes, torch.uint8)
+                    recvs.append((r_, recv))
+                    ops += [dist.P2POp(dist.isend, self._to_host(s_, nbytes, torch.uint8), peer, self.group),
+                            dist.P2POp(dist.irecv, recv, peer, self.group)]
             if ops:
                 for req in dist.batch_isend_irecv(ops):
                     req.wait()
+            for r_, recv in recvs:
+                self._from_host(r_, recv)
+            self._settle()
             return 0
         except Exception:  # pragma: no cover
             import traceback
@@ -175,9 +202,11 @@ class LibComm:
     def _allreduce(self, user, buf, count, op):
         try:
             dtype = torch.float32 if op in (0, 1) else torch.int32
-            t = self._host(buf, count * 4, dtype)
+            t = self._to_host(buf, count * 4, dtype)
             dist.all_reduce(t, op={0: dist.ReduceOp.MAX, 1: dist.ReduceOp.MIN, 2: dist.ReduceOp.MAX, 3: dist.ReduceOp.SUM}[op],
                             group=self.group)
+            self._from_host(buf, t)
+            self._settle()
             return 0
         except Exception:  # pragma: no cover
             import traceback
@@ -185,10 +214,12 @@ class LibComm:
             return 1
 
 
-def lib_comm(group=None) -> "LibComm":
-    key = id(group)
+def lib_comm(group=None, cuda: bool = False) -> "LibComm":
+    """The library's communicator for ``group`` (made once per group and memory kind); ``cuda``: the bands it connects
+    live in CUDA memory."""
+    key = (id(group), bool(cuda))
     if key not in _COMMS:
-        _COMMS[key] = LibComm(group)
+        _COMMS[key] = LibComm(group, cuda)
     return _COMMS[key]
 
 
@@ -284,7 +315,7 @@ def fill_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, solver_cls=None
             else:
                 height, row0 = h_, 0
         xr = C.c_int32(0)
-        cm = lib_comm(group)
+        cm = lib_comm(group, local_dem.is_cuda)
         _lib.check(_lib.lib().rdb200_mgpu_fill_depressions_d8_f32(cm.handle, local_dem.data_ptr(), w_, h_, int(g_top), int(g_bot),
                                                                   int(row0), int(height), C.byref(xr)))
         if return_stats:
@@ -455,7 +486,7 @@ def fa_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: float, di
         assert _on_device(acc) and acc.dtype == torch.float64 and acc.is_contiguous()
         _lib.use_torch_stream()
         xr = C.c_int32(0)
-        cm = lib_comm(group)
+        cm = lib_comm(group, local_dem.is_cuda)
         _lib.check(_lib.lib().rdb200_mgpu_fa_method_f32_f64(cm.handle, local_dem.data_ptr(), acc.data_ptr(), local_dem.shape[1],
                                                             local_dem.shape[0], float(nodata), int(g_top), int(g_bot), mid,
                                                             xparam, int(ones), C.byref(xr)))
@@ -581,7 +612,8 @@ class CudaFlatsBand:
         self._lib.check(self.L.rdb200_dev_flats_finish(self._state))
         self._state = None
 
-    # ---- seam payloads (comm-agnostic; used by the NCCL driver and by the single-GPU emulation) ----
+    # ---- seam payloads (comm-agnostic; the step-wise reference of the seam kernels of csrc/flats.cu, used by the
+    # one-device band emulation of the tests) ----
     def flag_payload(self, which: int):
         """uint8 rows [edge, ghost]: outlet flag of the component of every seam cell."""
         e, g = self.rows(which)
@@ -697,55 +729,16 @@ def _relax_band(solver, g_top, g_bot, rank, world, group, max_rounds=100000, sto
 
 def resolve_flats_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: float, group=None):
     """ResolveFlatsEpsilon over this rank's band, in place on the owned rows of ``local_dem`` (whose
-    ghost rows must hold the neighbours' elevation rows).  Collective.  Returns the number of seam
-    iterations (flags + heights)."""
-    rank = dist.get_rank(group) if dist.is_initialized() else 0
-    world = dist.get_world_size(group) if dist.is_initialized() else 1
-    F = CudaFlatsBand(local_dem, nodata, g_top, g_bot)
-
-    def exchange_ft():
-        if world == 1:
-            return
-        up = F.ft[F.rows(0)[0]].contiguous() if g_top else None
-        dn = F.ft[F.rows(1)[0]].contiguous() if g_bot else None
-        ru, rd = _neighbour_exchange(up, dn, g_top, g_bot, rank, group)
-        if ru is not None:
-            F.ft[0].copy_(ru[0])
-        if rd is not None:
-            F.ft[F.h - 1].copy_(rd[0])
-
-    def merge_until_stable(payload, merge):
-        it = 0
-        while world > 1:
-            it += 1
-            up = payload(0) if g_top else None
-            dn = payload(1) if g_bot else None
-            ru, rd = _neighbour_exchange(up, dn, g_top, g_bot, rank, group)
-            ch = False
-            if ru is not None:
-                ch |= merge(0, ru[0])
-            if rd is not None:
-                ch |= merge(1, rd[0])
-            flag = torch.tensor([1 if ch else 0], dtype=torch.int32, device=local_dem.device)
-            dist.all_reduce(flag, op=dist.ReduceOp.MAX, group=group)
-            if int(flag.item()) == 0:
-                break
-        return it
-
-    exchange_ft()               # IS_A_FLAT / NoData of the ghost rows
-    F.step("edges")
-    exchange_ft()               # low / high edge bits of the ghost rows
-    F.step("components")
-    iters = merge_until_stable(F.flag_payload, F.merge_flags)
-    F.step("labels")
-    for away in (True, False):
-        solver = F.gradient_begin(away)
-        from . import _lib
-        with _lib.scoped_param("fill_band_rounds", 64 if world > 1 else 0):  # (put back afterwards: a process-wide switch)
-            _relax_band(solver, g_top, g_bot, rank, world, group)
-        F.gradient_end(away, solver)
-        if away:
-            iters += merge_until_stable(F.height_payload, F.merge_heights)
-    F.step("apply")
-    F.finish()
-    return iters
+    ghost rows must hold the neighbours' elevation rows; on return they hold the neighbours' resolved
+    edge rows, so :func:`fa_band` can follow without :func:`exchange_rows`).  Collective.  Returns the
+    number of seam iterations (flags + heights).  The protocol runs in C++ over the library's
+    communicator (csrc/flats.cu: mgpu_resolve_flats_band)."""
+    from . import _lib
+    assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
+    _lib.use_torch_stream()
+    h, w = local_dem.shape
+    it = C.c_int32(0)
+    cm = lib_comm(group, local_dem.is_cuda)
+    _lib.check(_lib.lib().rdb200_mgpu_resolve_flats_epsilon_f32(cm.handle, local_dem.data_ptr(), w, h, float(nodata), int(g_top),
+                                                                int(g_bot), C.byref(it)))
+    return int(it.value)
