@@ -252,6 +252,9 @@ RDB200_API int rdb200_dev_generate_fbm_f32(float *d_dem, int32_t width, int32_t 
  *            rdb200_mgpu_fill_depressions_d8_f32(comm, d_band, W, rows, gt, gb, row0, H, NULL);
  *            rdb200_mgpu_resolve_flats_epsilon_f32(comm, d_band, W, rows, nodata, gt, gb, NULL);
  *            rdb200_mgpu_fa_f32_f64(comm, d_band, d_accum, W, rows, nodata, gt, gb, 0, 1, NULL);
+ *   or, for the direction-grid pipeline after the fill (uint8 directions and int32 upslope-cell counts):
+ *            rdb200_mgpu_d8_flow_directions_flats_f32(comm, d_band, d_dirs, W, rows, nodata, gt, gb, 0, NULL);
+ *            rdb200_mgpu_d8_flow_accum_u8_i32(comm, d_dirs, d_area, W, rows, gt, gb, NULL);
  */
 typedef struct rdb200_comm rdb200_comm;
 enum { RDB200_MAX_F32 = 0, RDB200_MIN_F32 = 1, RDB200_MAX_I32 = 2, RDB200_SUM_I32 = 3 };
@@ -297,6 +300,24 @@ RDB200_API int rdb200_mgpu_fa_method_f32_f64(const rdb200_comm *comm, const floa
                                              int32_t width, int32_t local_rows, float nodata, int32_t ghost_top,
                                              int32_t ghost_bottom, int32_t method, double xparam, int32_t accum_is_ones,
                                              int32_t *exchange_rounds);
+/* barnes_flat_resolution_d8 (include/richdem/flats/flat_resolution.hpp:588-607) over row bands: writes the D8 directions
+ * of the band into d_band_dirs (local_rows x width, like d_band_dem).  The ghost rows of d_band_dem must hold the
+ * neighbours' edge rows on entry, as the band fill leaves them.  The owned rows equal the single-GPU
+ * rdb200_d8_flow_directions_flats_f32 of the whole raster, bit for bit; with alter = 1 so do the owned rows of the altered
+ * d_band_dem.  On return the ghost rows of d_band_dirs (and, with alter = 1, of d_band_dem) hold the neighbours' edge
+ * rows.  Argument checks as rdb200_mgpu_resolve_flats_epsilon_f32, d_band_dirs included.  *seam_iterations (optional):
+ * rounds of the outlet-flag and flat-height merges across seams (0 for one band). */
+RDB200_API int rdb200_mgpu_d8_flow_directions_flats_f32(const rdb200_comm *comm, float *d_band_dem, uint8_t *d_band_dirs,
+                                                        int32_t width, int32_t local_rows, float nodata, int32_t ghost_top,
+                                                        int32_t ghost_bottom, int32_t alter, int32_t *seam_iterations);
+/* d8_flow_accum (include/richdem/methods/d8_methods.hpp:47-139) of a uint8 D8 direction grid cut into row bands.  The
+ * ghost rows of d_band_dirs are not read: the call exchanges the edge rows itself.  The owned rows of d_band_area equal
+ * the single-GPU rdb200_d8_flow_accum_u8_i32 of the whole grid (NoData 255 -> -1; codes other than 0..8 / 255 carry no
+ * flow); its ghost rows are scratch.  Argument checks as rdb200_mgpu_resolve_flats_epsilon_f32.  *exchange_rounds
+ * (optional): walk rounds, each followed by one exchange of the flow that crossed a seam. */
+RDB200_API int rdb200_mgpu_d8_flow_accum_u8_i32(const rdb200_comm *comm, const uint8_t *d_band_dirs, int32_t *d_band_area,
+                                                int32_t width, int32_t local_rows, int32_t ghost_top, int32_t ghost_bottom,
+                                                int32_t *exchange_rounds);
 
 /* ---- row-band (multi-GPU) fill: one band per GPU, halo rows exchanged by the caller -- */
 /* The band raster handed in is (band_rows + ghost rows) x width.  Its first and last rows are

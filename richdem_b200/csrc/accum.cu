@@ -2111,6 +2111,40 @@ __global__ void __launch_bounds__(256) band_mark_sources_props_kernel(const floa
   else if ((st[i] & kDepsMask) == 0) st[i] = kSrcFlag;
 }
 
+// ---- direction grids (d8_flow_accum) over row bands ----
+// unit weights: ghost rows become empty parking slots, NoData cells -1 (d8_methods.hpp:71-74, :111)
+__global__ void __launch_bounds__(256) band_init_dirs_accum_kernel(const uint8_t *__restrict__ code, double *accum, int W, int H,
+                                                                    int y_lo, int y_hi) {
+  const size_t n = (size_t)W * H;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int y = (int)(i / W);
+  accum[i] = (y < y_lo || y >= y_hi) ? 0.0 : (code[i] == kCodeNoData ? -1.0 : 1.0);
+}
+
+// (only directions 1..8 are cleared, and only NoData (255) is tested at the receiver: concurrent clears are harmless)
+__global__ void __launch_bounds__(256) band_settle_dir_codes_kernel(uint8_t *code, int W, int H) {
+  const size_t n = (size_t)W * H;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int d = code[i];
+  if (d == 0 || d > 8) return;
+  const int y = (int)(i / W), x = (int)(i - (size_t)y * W);
+  const int nx = x + d8dx(d), ny = y + d8dy(d);
+  if (nx < 0 || ny < 0 || nx >= W || ny >= H || code[(size_t)ny * W + nx] == kCodeNoData) code[i] = 0;
+}
+
+// the int32 areas from the accumulator: doubles, or -- packed words of cells that never completed, which only a cycle
+// in the direction grid leaves behind -- [donors left (1..8) | integer sum], the partial sum d8_flow_accum leaves there
+__global__ void __launch_bounds__(256) band_area_from_accum_kernel(const unsigned long long *__restrict__ word,
+                                                                    int32_t *__restrict__ area, size_t n, int packed) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long v = word[i];
+  const unsigned top = (unsigned)(v >> 56);
+  area[i] = (packed && top >= 1 && top <= 8) ? (int32_t)(v & kPkVal) : (int32_t)__longlong_as_double((long long)v);
+}
+
 }  // namespace
 
 // Flow accumulation methods of the band entry points, numbered as rdb200_dev_fa_method_f32_f64: 0 D8, 1 Tarboton,
@@ -2228,6 +2262,46 @@ struct FaccState {
     band_init_props_accum_kernel<<<blocks, 256, 0, c.stream>>>(props.p, accum, W, H, gt, H - gb, ones ? 1 : 0);
     RDB_CK(cudaGetLastError());
     count_launch(2);
+  }
+
+  // d8_flow_accum of a direction grid (unit weights): the codes are the directions, codes other than 0..8 / NoData
+  // meaning no flow.  settle_dir_codes() must follow once the ghost rows hold the neighbours' codes.
+  void begin_dirs(const uint8_t *d_dirs, double *d_accum, int w, int h, int ghost_top, int ghost_bottom) {
+    Ctx &c = ctx();
+    W = w;
+    H = h;
+    gt = ghost_top ? 1 : 0;
+    gb = ghost_bottom ? 1 : 0;
+    accum = d_accum;
+    from_dirs = true;
+    if (h - gt - gb < 1) fail("facc_begin: band has no owned rows");
+    packed = (w & 3) == 0 && ((uintptr_t)d_accum & 15) == 0 && c.params.accum_packed != 0;
+    code.alloc(n());
+    if (!packed) st.alloc(n());
+    ghostcnt.alloc(2 * (size_t)W);
+    fr0.alloc(n());
+    fr1.alloc(n());
+    cnt.alloc(4);
+    RDB_CK(cudaMemsetAsync(ghostcnt.p, 0, 2 * (size_t)W * sizeof(int), c.stream));
+    RDB_CK(cudaMemsetAsync(cnt.p, 0, 4 * sizeof(int), c.stream));
+    const unsigned blocks = (unsigned)((n() + 255) / 256);
+    sanitize_dirs_kernel<<<blocks, 256, 0, c.stream>>>(d_dirs, code.p, n());
+    // the packed gather (first run) initialises every accumulator word
+    if (!packed) band_init_dirs_accum_kernel<<<blocks, 256, 0, c.stream>>>(code.p, accum, W, H, gt, H - gb);
+    RDB_CK(cudaGetLastError());
+    count_launch(packed ? 1 : 2);
+  }
+  bool from_dirs = false;
+
+  // A direction that leaves the local raster or points at a NoData cell becomes "no flow".  For an owned cell that is
+  // exactly the flow d8_flow_accum drops: off the global raster (a seam row is inside the local raster) or into NoData,
+  // a NoData ghost cell included.  For a ghost cell it only drops flow that never reaches this band.  The walks then
+  // need no bounds test and never add into a NoData word, as with codes computed from a DEM.
+  void settle_dir_codes() {
+    Ctx &c = ctx();
+    band_settle_dir_codes_kernel<<<(unsigned)((n() + 255) / 256), 256, 0, c.stream>>>(code.p, W, H);
+    RDB_CK(cudaGetLastError());
+    count_launch();
   }
 
   int edge_row(int which) const { return which == 0 ? gt : H - 1 - gb; }   // my first / last owned row
@@ -2532,17 +2606,14 @@ void FaccState::sum_rows(int *d_sums) {
 // protocol of FaccState (edge codes -- or, for proportions, seam donor masks -- to the neighbours once, then rounds of:
 // walk | parked outflow of the two seams in ONE message per neighbour (sums and parcel counts) | neighbours' inflow
 // releases cells of the edge rows | a 1-int all-reduce says whether anyone shipped).
-void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, int w, int hloc, float nodata, int gt, int gb,
-                  int method, double xparam, bool ones, int *xrounds) {
+static void fa_band_rounds(const rdb200_comm *comm, FaccState &A, int *xrounds) {
   Ctx &c = ctx();
   const int world = comm_world(comm);
-  FaccState A;
-  A.begin(d_dem, d_accum, w, hloc, nodata, gt, gb, method, xparam, ones);
-  gt = A.gt;
-  gb = A.gb;
+  const int w = A.W, gt = A.gt, gb = A.gb;
   // message layout per side: [w doubles: sums | w ints: parcel counts]; codes: [w floats: rmax | w bytes: codes or seam
-  // donor masks] (the float half is unused for proportions)
-  const size_t msg = (size_t)w * 12;
+  // donor masks] (the float half is unused for proportions).  Each of the four messages starts 16-byte aligned, so that
+  // the sums of the second one are aligned doubles for an odd width too.
+  const size_t msg = ((size_t)w * 12 + 15) & ~(size_t)15;
   DevBuf<uint8_t> buf(4 * msg);
   uint8_t *su = buf.p, *sd = buf.p + msg, *ru = buf.p + 2 * msg, *rd = buf.p + 3 * msg;
   auto rmaxp = [&](uint8_t *m) { return reinterpret_cast<float *>(m); };
@@ -2557,6 +2628,7 @@ void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, 
     if (gt) A.set_ghost_codes(0, codep(ru), rmaxp(ru));
     if (gb) A.set_ghost_codes(1, codep(rd), rmaxp(rd));
   }
+  if (A.from_dirs) A.settle_dir_codes();
   DevBuf<int> flag(1);
   int *hflag = (int *)c.pinned + 1024;
   int rounds = 0;
@@ -2614,6 +2686,37 @@ void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, 
   }
   RDB_CK(cudaStreamSynchronize(c.stream));
   if (xrounds) *xrounds = rounds;
+}
+
+void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, int w, int hloc, float nodata, int gt, int gb,
+                  int method, double xparam, bool ones, int *xrounds) {
+  FaccState A;
+  A.begin(d_dem, d_accum, w, hloc, nodata, gt, gb, method, xparam, ones);
+  fa_band_rounds(comm, A, xrounds);
+}
+
+// d8_flow_accum over row bands: the protocol above on the codes of a direction grid, whose ghost rows are not trusted
+// (the edge-code exchange installs the neighbours' rows).  The walk runs on a float64 accumulator -- packed
+// [donors | integer sum] words where the width allows -- and the int32 areas are written at the end; the ghost rows of
+// d_area are scratch.
+void mgpu_d8_flow_accum_band(const rdb200_comm *comm, const uint8_t *d_dirs, int32_t *d_area, int w, int hloc, int gt, int gb,
+                             int *xrounds) {
+  Ctx &c = ctx();
+  const char *what = "mgpu_d8_flow_accum";
+  if (!d_area) fail("%s: null pointer", what);
+  check_band_args(what, comm, d_dirs, w, hloc, gt, gb);
+  const size_t n = (size_t)w * hloc;
+  DevBuf<double> acc(n);
+  {
+    FaccState A;
+    A.begin_dirs(d_dirs, acc.p, w, hloc, gt, gb);
+    fa_band_rounds(comm, A, xrounds);
+    band_area_from_accum_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(
+        reinterpret_cast<const unsigned long long *>(acc.p), d_area, n, A.packed ? 1 : 0);
+    RDB_CK(cudaGetLastError());
+    count_launch();
+  }
+  RDB_CK(cudaStreamSynchronize(c.stream));
 }
 
 void capi_set_error(const char *msg);

@@ -637,4 +637,31 @@ int rdb200_mgpu_resolve_flats_epsilon_f32(const rdb200_comm *comm, float *d_band
   CAPI_END
 }
 
+int rdb200_mgpu_d8_flow_directions_flats_f32(const rdb200_comm *comm, float *d_band_dem, uint8_t *d_band_dirs, int32_t w,
+                                             int32_t rows, float nodata, int32_t gt, int32_t gb, int32_t alter,
+                                             int32_t *seam_iterations) {
+  int it = 0;
+  CAPI_TRY
+  if (!comm || !d_band_dem || !d_band_dirs) fail("mgpu_d8_flow_directions_flats: null pointer");
+  check_dims(w, rows);
+  CallScope cs((int64_t)w * rows);
+  mgpu_d8_flow_directions_flats_band(comm, d_band_dem, d_band_dirs, w, rows, nodata, gt, gb, alter != 0, &it);
+  cs.done();
+  if (seam_iterations) *seam_iterations = it;
+  CAPI_END
+}
+
+int rdb200_mgpu_d8_flow_accum_u8_i32(const rdb200_comm *comm, const uint8_t *d_band_dirs, int32_t *d_band_area, int32_t w,
+                                     int32_t rows, int32_t gt, int32_t gb, int32_t *exchange_rounds) {
+  int xr = 0;
+  CAPI_TRY
+  if (!comm || !d_band_dirs || !d_band_area) fail("mgpu_d8_flow_accum: null pointer");
+  check_dims(w, rows);
+  CallScope cs((int64_t)w * rows);
+  mgpu_d8_flow_accum_band(comm, d_band_dirs, d_band_area, w, rows, gt, gb, &xr);
+  cs.done();
+  if (exchange_rounds) *exchange_rounds = xr;
+  CAPI_END
+}
+
 }  // extern "C"

@@ -126,6 +126,24 @@ void comm_allreduce(const rdb200_comm *c, void *buf, size_t count, int op) {
   if (c->allreduce(c->user, buf, count, op) != 0) fail("multi-GPU: the caller's all-reduce callback failed");
 }
 
+// Arguments of a collective band driver.  Every driver calls this before its first collective: a rank that fails here
+// must not leave its peers waiting.
+void check_band_args(const char *what, const rdb200_comm *comm, const void *d_band, int w, int hloc, int gt, int gb) {
+  const int rank = comm_rank(comm), world = comm_world(comm);
+  if (!comm || !d_band) fail("%s: null pointer", what);
+  if (w < 1 || hloc - (gt ? 1 : 0) - (gb ? 1 : 0) < 1) fail("%s: band has no owned rows (%d x %d)", what, w, hloc);
+  if ((gt != 0) != (rank > 0) || (gb != 0) != (rank < world - 1))
+    fail("%s: rank %d of %d needs ghost_top = %d and ghost_bottom = %d (got %d, %d)", what, rank, world, rank > 0 ? 1 : 0,
+         rank < world - 1 ? 1 : 0, gt, gb);
+}
+
+// one edge row of a band array (elem bytes per cell) to each neighbour's ghost row, in place
+void exchange_band_rows(const rdb200_comm *comm, void *d_band, size_t elem, int w, int hloc, int gt, int gb) {
+  uint8_t *b = static_cast<uint8_t *>(d_band);
+  const size_t row = (size_t)w * elem;
+  comm_exchange(comm, b + (size_t)gt * row, b, b + (size_t)(hloc - 1 - gb) * row, b + (size_t)(hloc - 1) * row, row);
+}
+
 void capi_set_error(const char *msg);
 
 }  // namespace rdb

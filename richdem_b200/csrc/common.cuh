@@ -160,12 +160,18 @@ int comm_rank(const rdb200_comm *c);
 int comm_world(const rdb200_comm *c);
 void comm_exchange(const rdb200_comm *c, const void *send_up, void *recv_up, const void *send_dn, void *recv_dn, size_t bytes);
 void comm_allreduce(const rdb200_comm *c, void *buf, size_t count, int op);
+void check_band_args(const char *what, const rdb200_comm *comm, const void *d_band, int w, int hloc, int gt, int gb);
+void exchange_band_rows(const rdb200_comm *comm, void *d_band, size_t elem, int w, int hloc, int gt, int gb);
 void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, int gt, int gb, int row0, int H, int *xrounds);
 // method: 0 D8, 1 Tarboton, 2 D4, 3 Holmgren (xparam; Quinn = 1.0), 4 Freeman (xparam)
 void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, int w, int hloc, float nodata, int gt, int gb,
                   int method, double xparam, bool ones, int *xrounds);
 void mgpu_resolve_flats_band(const rdb200_comm *comm, float *d_local, int w, int hloc, float nodata, int gt, int gb,
                              int *seam_iters);
+void mgpu_d8_flow_directions_flats_band(const rdb200_comm *comm, float *d_dem, uint8_t *d_dirs, int w, int hloc, float nodata,
+                                        int gt, int gb, bool alter, int *seam_iters);
+void mgpu_d8_flow_accum_band(const rdb200_comm *comm, const uint8_t *d_dirs, int32_t *d_area, int w, int hloc, int gt, int gb,
+                             int *xrounds);
 // the band relaxation protocol over a state that holds its start; R sweep rounds between halo exchanges (0: none)
 int mgpu_relax_band(const rdb200_comm *comm, rdb200_fill_state *state, int gt, int gb, int R);
 

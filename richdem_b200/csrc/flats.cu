@@ -943,8 +943,11 @@ __global__ void __launch_bounds__(256) seam_merge_heights_kernel(const int *__re
   if (v > Hh[lab - 1] && atomicMax(&Hh[lab - 1], v) < v) *changed = 1;  // (heights only grow: a stale read only lets more through)
 }
 
-// ---- the steps (shared by the C++ band driver and the step-wise entry points) ----
-rdb200_flats_state *flats_begin(float *d_dem, int width, int height, float nodata, int ghost_top, int ghost_bottom) {
+// ---- the steps (shared by the C++ band drivers and the step-wise entry points) ----
+// d_dirs: classify from a direction grid (flats_from_dirs_kernel: flags and edge bits in one pass) instead of from the
+// elevations
+rdb200_flats_state *flats_begin(float *d_dem, int width, int height, float nodata, int ghost_top, int ghost_bottom,
+                                const uint8_t *d_dirs = nullptr) {
   Ctx &c = ctx();
   auto *s = new rdb200_flats_state();
   try {
@@ -967,7 +970,10 @@ rdb200_flats_state *flats_begin(float *d_dem, int width, int height, float nodat
     RDB_CK(cudaMemsetAsync(s->rootflag.p, 0, n, c.stream));
     RDB_CK(cudaMemsetAsync(s->Hh.p, 0, n * sizeof(int), c.stream));
     // rows 0 / H-1 are classified as raster-edge cells; for ghost rows the caller overwrites them
-    flats_classify_kernel<<<s->blocks(), 256, 0, c.stream>>>(d_dem, s->ft.p, width, height, nodata, s->dev.p);
+    if (d_dirs)
+      flats_from_dirs_kernel<<<c.num_sms * 16, 256, 0, c.stream>>>(d_dem, d_dirs, s->ft.p, width, height, s->dev.p);
+    else
+      flats_classify_kernel<<<s->blocks(), 256, 0, c.stream>>>(d_dem, s->ft.p, width, height, nodata, s->dev.p);
     RDB_CK(cudaGetLastError());
     RDB_CK(cudaStreamSynchronize(c.stream));
   } catch (...) {
@@ -1017,10 +1023,11 @@ void flats_gradient_end(rdb200_flats_state *s, bool away, rdb200_fill_state *dis
   RDB_CK(cudaStreamSynchronize(c.stream));
 }
 
-void flats_apply(rdb200_flats_state *s) {
+// d_mask_out: write the increment mask there and leave the elevations alone
+void flats_apply(rdb200_flats_state *s, int32_t *d_mask_out = nullptr) {
   Ctx &c = ctx();
-  flats_apply_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->dem, s->labels.p, s->away.p, s->tw.p, s->Hh.p, nullptr, nullptr, s->W,
-                                                        s->H, 1, s->dev.p);
+  flats_apply_kernel<<<s->blocks(), 256, 0, c.stream>>>(s->dem, s->labels.p, s->away.p, s->tw.p, s->Hh.p, d_mask_out, nullptr,
+                                                        s->W, s->H, d_mask_out ? 0 : 1, s->dev.p);
   RDB_CK(cudaGetLastError());
   FlatDev *hd = (FlatDev *)c.pinned;
   RDB_CK(cudaMemcpyAsync(hd, s->dev.p, sizeof(FlatDev), cudaMemcpyDeviceToHost, c.stream));
@@ -1028,35 +1035,19 @@ void flats_apply(rdb200_flats_state *s) {
   if (hd->dist_overflow) fail("resolve_flats (band): a flat is more than 2^24 cells long; float distances are not exact there");
 }
 
-}  // namespace
-
-// ResolveFlatsEpsilon over row bands, driven from C++ over a rdb200_comm: the protocol above, in that order.  Flag rows
-// go straight from the flag array into the neighbours' ghost rows; the seam merges are the kernels above, and a merge
-// loop ends when a 1-int MAX all-reduce says that no rank's merge changed anything.  The two gradients are band
-// relaxations (mgpu_relax_band) of the distance states, with R = 64 sweep rounds between halo exchanges when there are
-// several bands.  On return the ghost rows of d_local hold the neighbours' resolved edge rows (one last exchange), so
-// that accumulation can follow without another one.  *seam_iters: flag + height merge iterations (0 for one band).
-void mgpu_resolve_flats_band(const rdb200_comm *comm, float *d_local, int w, int hloc, float nodata, int gt, int gb,
-                             int *seam_iters) {
+// The band protocol of a begun state up to the increment mask, in the order of the comment above.  Flag rows go straight
+// from the flag array into the neighbours' ghost rows; the seam merges are the kernels above, and a merge loop ends when
+// a 1-int MAX all-reduce says that no rank's merge changed anything.  The two gradients are band relaxations
+// (mgpu_relax_band) of the distance states, with R = 64 sweep rounds between halo exchanges when there are several
+// bands.  A state begun from a direction grid already has its edge bits (its ghost rows held the neighbours'
+// directions), so one flag exchange suffices.  Returns the flag + height merge iterations (0 for one band).
+int flats_band_steps(const rdb200_comm *comm, rdb200_flats_state *s, bool from_dirs) {
   Ctx &c = ctx();
-  const int rank = comm_rank(comm), world = comm_world(comm);
-  // every check comes before the first collective: a rank that fails here must not leave its peers waiting
-  if (!comm || !d_local) fail("mgpu_resolve_flats: null pointer");
-  if (w < 1 || hloc - (gt ? 1 : 0) - (gb ? 1 : 0) < 1) fail("mgpu_resolve_flats: band has no owned rows (%d x %d)", w, hloc);
-  if ((gt != 0) != (rank > 0) || (gb != 0) != (rank < world - 1))
-    fail("mgpu_resolve_flats: rank %d of %d needs ghost_top = %d and ghost_bottom = %d (got %d, %d)", rank, world, rank > 0 ? 1 : 0,
-         rank < world - 1 ? 1 : 0, gt, gb);
-  gt = gt ? 1 : 0;
-  gb = gb ? 1 : 0;
-  std::unique_ptr<rdb200_flats_state> s(flats_begin(d_local, w, hloc, nodata, gt, gb));
+  const int world = comm_world(comm);
+  const int w = s->W, hloc = s->H, gt = s->gt, gb = s->gb;
   const int edge[2] = {gt, hloc - 1 - gb}, ghost[2] = {0, hloc - 1};  // per side: 0 = top, 1 = bottom
   const bool side_on[2] = {gt != 0, gb != 0};
-  // one edge row of `p` (elem bytes per cell) to each neighbour's ghost row, in place
-  auto exchange_rows = [&](void *p, size_t elem) {
-    uint8_t *b = static_cast<uint8_t *>(p);
-    const size_t row = (size_t)w * elem;
-    comm_exchange(comm, b + edge[0] * row, b + ghost[0] * row, b + edge[1] * row, b + ghost[1] * row, row);
-  };
+  auto exchange_rows = [&](void *p, size_t elem) { exchange_band_rows(comm, p, elem, w, hloc, gt, gb); };
   // message buffers: send up, send down, receive up, receive down; 2 rows of int32 at most
   const size_t msg = (size_t)w * 2 * sizeof(int);
   DevBuf<uint8_t> buf(4 * msg);
@@ -1100,26 +1091,85 @@ void mgpu_resolve_flats_band(const rdb200_comm *comm, float *d_local, int w, int
   };
   const int R = world > 1 ? 64 : 0;  // sweep rounds between halo exchanges (0: one band relaxes to its fixed point)
 
-  exchange_rows(s->ft.p, 1);  // IS_A_FLAT / NoData of the ghost rows
-  flats_edges(s.get());
-  exchange_rows(s->ft.p, 1);  // low / high edge bits of the ghost rows
-  flats_components(s.get());
+  exchange_rows(s->ft.p, 1);  // IS_A_FLAT / NoData (and, from directions, edge bits) of the ghost rows
+  if (!from_dirs) {
+    flats_edges(s);
+    exchange_rows(s->ft.p, 1);  // low / high edge bits of the ghost rows
+  }
+  flats_components(s);
   int iters = merge_until_stable(false);  // (labels holds every cell's root until flats_labels)
-  flats_labels(s.get());
+  flats_labels(s);
   for (const bool away : {true, false}) {
-    rdb200_fill_state *ds = flats_gradient_begin(s.get(), away);
+    rdb200_fill_state *ds = flats_gradient_begin(s, away);
     try {
       mgpu_relax_band(comm, ds, gt, gb, R);
     } catch (...) {
       rdb200_dev_fill_finish(ds, nullptr);
       throw;
     }
-    flats_gradient_end(s.get(), away, ds);
+    flats_gradient_end(s, away, ds);
     if (away) iters += merge_until_stable(true);
   }
+  return iters;
+}
+
+}  // namespace
+
+// ResolveFlatsEpsilon over row bands, driven from C++ over a rdb200_comm.  On return the ghost rows of d_local hold the
+// neighbours' resolved edge rows (one last exchange), so that accumulation can follow without another one.
+// *seam_iters: flag + height merge iterations (0 for one band).
+void mgpu_resolve_flats_band(const rdb200_comm *comm, float *d_local, int w, int hloc, float nodata, int gt, int gb,
+                             int *seam_iters) {
+  Ctx &c = ctx();
+  check_band_args("mgpu_resolve_flats", comm, d_local, w, hloc, gt, gb);
+  gt = gt ? 1 : 0;
+  gb = gb ? 1 : 0;
+  std::unique_ptr<rdb200_flats_state> s(flats_begin(d_local, w, hloc, nodata, gt, gb));
+  const int iters = flats_band_steps(comm, s.get(), false);
   flats_apply(s.get());
   s.reset();
-  exchange_rows(d_local, sizeof(float));  // the neighbours' resolved edge rows
+  exchange_band_rows(comm, d_local, sizeof(float), w, hloc, gt, gb);  // the neighbours' resolved edge rows
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  if (seam_iters) *seam_iters = iters;
+}
+
+// barnes_flat_resolution_d8 (d8_flow_directions_flats_dev) over row bands.  The DEM's ghost rows hold the neighbours'
+// edge rows on entry.  Plain directions of the local raster first: its rows 0 / H-1 get the raster-edge rule, which is
+// right for the global top / bottom row and is replaced by the neighbours' directions in a ghost row.  The flats are
+// classified from the directions and resolved by the band protocol.  alter = 0: the increment mask crosses the seams
+// (d8_flow_flats compares a cell's mask with its same-label neighbours', ghost cells included; adjacent cells share a
+// local label exactly when they share a flat), then the NO_FLOW cells of the owned rows take their masked directions.
+// alter = 1: the increments go into the owned rows of the DEM, its edge rows cross the seams and the directions are
+// computed again.  On return the ghost rows of d_dirs (and, with alter = 1, of d_dem) hold the neighbours' edge rows.
+void mgpu_d8_flow_directions_flats_band(const rdb200_comm *comm, float *d_dem, uint8_t *d_dirs, int w, int hloc, float nodata,
+                                        int gt, int gb, bool alter, int *seam_iters) {
+  Ctx &c = ctx();
+  const char *what = "mgpu_d8_flow_directions_flats";
+  if (!d_dirs) fail("%s: null pointer", what);
+  check_band_args(what, comm, d_dem, w, hloc, gt, gb);
+  gt = gt ? 1 : 0;
+  gb = gb ? 1 : 0;
+  auto exchange_rows = [&](void *p, size_t elem) { exchange_band_rows(comm, p, elem, w, hloc, gt, gb); };
+  d8_flow_directions_dev(d_dem, d_dirs, w, hloc, nodata);
+  exchange_rows(d_dirs, 1);
+  std::unique_ptr<rdb200_flats_state> s(flats_begin(d_dem, w, hloc, nodata, gt, gb, d_dirs));
+  const int iters = flats_band_steps(comm, s.get(), true);
+  if (alter) {
+    flats_apply(s.get());
+    s.reset();
+    exchange_rows(d_dem, sizeof(float));
+    d8_flow_directions_dev(d_dem, d_dirs, w, hloc, nodata);
+  } else {
+    DevBuf<int32_t> mask((size_t)w * hloc);
+    flats_apply(s.get(), mask.p);
+    exchange_rows(mask.p, sizeof(int32_t));
+    d8_flow_flats_kernel<<<c.num_sms * 16, 256, 0, c.stream>>>(mask.p, s->labels.p, d_dirs, w, hloc);
+    RDB_CK(cudaGetLastError());
+    count_launch();
+    RDB_CK(cudaStreamSynchronize(c.stream));
+    s.reset();
+  }
+  exchange_rows(d_dirs, 1);
   RDB_CK(cudaStreamSynchronize(c.stream));
   if (seam_iters) *seam_iters = iters;
 }

@@ -742,3 +742,41 @@ def resolve_flats_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata
     _lib.check(_lib.lib().rdb200_mgpu_resolve_flats_epsilon_f32(cm.handle, local_dem.data_ptr(), w, h, float(nodata), int(g_top),
                                                                 int(g_bot), C.byref(it)))
     return int(it.value)
+
+
+# =================================================================================================
+# The direction-grid pipeline over row bands (FlowDirectionsD8Resolved -> D8FlowAccum)
+# =================================================================================================
+def d8_flow_directions_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: float, alter: bool = False,
+                            group=None):
+    """FlowDirectionsD8Resolved over this rank's band.  ``local_dem`` is (g_top + owned + g_bot) x W and its ghost rows
+    must hold the neighbours' elevation rows (:func:`fill_band` leaves them so).  ``alter=True`` raises the flat cells of
+    the owned rows in place, as on one GPU.  Collective.  Returns (uint8 directions of the same local shape, whose ghost
+    rows hold the neighbours' edge-row directions, seam iterations)."""
+    from . import _lib
+    assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
+    _lib.use_torch_stream()
+    h, w = local_dem.shape
+    dirs = torch.empty((h, w), dtype=torch.uint8, device=local_dem.device)
+    it = C.c_int32(0)
+    cm = lib_comm(group, local_dem.is_cuda)
+    _lib.check(_lib.lib().rdb200_mgpu_d8_flow_directions_flats_f32(cm.handle, local_dem.data_ptr(), dirs.data_ptr(), w, h,
+                                                                   float(nodata), int(g_top), int(g_bot), int(bool(alter)),
+                                                                   C.byref(it)))
+    return dirs, int(it.value)
+
+
+def d8_flow_accum_band(local_dirs: "torch.Tensor", g_top: int, g_bot: int, group=None):
+    """D8FlowAccum over this rank's band of a uint8 direction grid, (g_top + owned + g_bot) x W.  Its ghost rows are not
+    read (the edge rows are exchanged here).  Collective.  Returns (int32 upslope-cell counts of the same local shape,
+    ghost rows scratch, exchange rounds)."""
+    from . import _lib
+    assert _on_device(local_dirs) and local_dirs.dtype == torch.uint8 and local_dirs.is_contiguous()
+    _lib.use_torch_stream()
+    h, w = local_dirs.shape
+    area = torch.empty((h, w), dtype=torch.int32, device=local_dirs.device)
+    xr = C.c_int32(0)
+    cm = lib_comm(group, local_dirs.is_cuda)
+    _lib.check(_lib.lib().rdb200_mgpu_d8_flow_accum_u8_i32(cm.handle, local_dirs.data_ptr(), area.data_ptr(), w, h, int(g_top),
+                                                           int(g_bot), C.byref(xr)))
+    return area, int(xr.value)

@@ -1,5 +1,6 @@
 """Multi-GPU check (run under torchrun on N GPUs): sharded fill + FA_D8 / FA_Dinf over NCCL must
 equal the single-GPU answer computed on rank 0.  Writes gpurun_out/mgpu_check_<N>.json."""
+# Also checked: flat resolution, and the direction pipeline on the filled raster (resolved D8 directions, d8_flow_accum).
 import json, os, sys, time
 import numpy as np
 import torch
@@ -27,6 +28,7 @@ for (H, W, q) in [(3000, 2000, 0.5), (8192, 8192, 0.0)]:
     filled, frounds = sharded.fill_band(loc.clone(), gt, gb, multigrid=MG, row0=r0 - gt, height=H, vcycle=VC)
     torch.cuda.synchronize(); dist.barrier(); tf = time.time() - t; t = time.time()
     own_f = filled[gt:gt + (r1 - r0)].clone()
+    filled_band = filled.clone()
     # flat resolution over bands (in place), then refresh the ghost rows with the neighbours' resolved rows
     seam_iters = sharded.resolve_flats_band(filled, gt, gb, ND)
     sharded.exchange_rows(filled, gt, gb)
@@ -35,7 +37,13 @@ for (H, W, q) in [(3000, 2000, 0.5), (8192, 8192, 0.0)]:
     acc, arounds = sharded.fa_band(filled, gt, gb, ND, dinf=False)
     torch.cuda.synchronize(); dist.barrier(); ta = time.time() - t; t = time.time()
     accinf, irounds = sharded.fa_band(filled, gt, gb, ND, dinf=True)
-    torch.cuda.synchronize(); dist.barrier(); ti = time.time() - t
+    torch.cuda.synchronize(); dist.barrier(); ti = time.time() - t; t = time.time()
+    # the direction-grid pipeline on the filled band (its ghost rows hold the neighbours' filled rows)
+    dirs, dseam = sharded.d8_flow_directions_band(filled_band, gt, gb, ND)
+    area, drounds = sharded.d8_flow_accum_band(dirs, gt, gb)
+    torch.cuda.synchronize(); dist.barrier(); td = time.time() - t
+    own_d = dirs[gt:gt + (r1 - r0)].contiguous()
+    own_ar = area[gt:gt + (r1 - r0)].contiguous()
     # single-GPU truth on rank 0
     own_a = acc[gt:gt + (r1 - r0)].contiguous()
     own_i = accinf[gt:gt + (r1 - r0)].contiguous()
@@ -44,6 +52,11 @@ for (H, W, q) in [(3000, 2000, 0.5), (8192, 8192, 0.0)]:
         _lib.check(L.rdb200_dev_generate_fbm_f32(full.data_ptr(), W, H, 0, 7, 12, q))
         _lib.check(L.rdb200_dev_fill_depressions_d8_f32(full.data_ptr(), W, H))
         full_filled = full.clone()
+        d1, z1 = torch.empty((H, W), dtype=torch.uint8, device="cuda"), full_filled.clone()
+        _lib.check(L.rdb200_dev_d8_flow_directions_flats_f32(z1.data_ptr(), d1.data_ptr(), W, H, ND, 0))
+        del z1
+        ar1 = torch.empty((H, W), dtype=torch.int32, device="cuda")
+        _lib.check(L.rdb200_dev_d8_flow_accum_u8_i32(d1.data_ptr(), ar1.data_ptr(), W, H))
         _lib.check(L.rdb200_dev_resolve_flats_epsilon_f32(full.data_ptr(), W, H, ND))
         a1 = torch.empty((H, W), dtype=torch.float64, device="cuda")
         _lib.check(L.rdb200_dev_fa_d8_f32_f64(full.data_ptr(), a1.data_ptr(), W, H, ND, 1))
@@ -51,9 +64,9 @@ for (H, W, q) in [(3000, 2000, 0.5), (8192, 8192, 0.0)]:
         _lib.check(L.rdb200_dev_fa_tarboton_f32_f64(full.data_ptr(), a2.data_ptr(), W, H, ND, 1))
     ok = {}
     for name, own, dtype in (("fill", own_f, torch.float32), ("flats", own_r, torch.float32), ("fa_d8", own_a, torch.float64),
-                             ("fa_dinf", own_i, torch.float64)):
+                             ("fa_dinf", own_i, torch.float64), ("d8_dirs", own_d, torch.uint8), ("d8_area", own_ar, torch.int32)):
         if rank == 0:
-            ref = {"fill": full_filled, "flats": full, "fa_d8": a1, "fa_dinf": a2}[name]
+            ref = {"fill": full_filled, "flats": full, "fa_d8": a1, "fa_dinf": a2, "d8_dirs": d1, "d8_area": ar1}[name]
             good = True
             for g in range(world):
                 b0, b1, _, _ = sharded.local_rows(H, world, g)
@@ -71,7 +84,8 @@ for (H, W, q) in [(3000, 2000, 0.5), (8192, 8192, 0.0)]:
             dist.send(own, 0)
     if rank == 0:
         case = {"H": H, "W": W, "q": q, "ok": ok, "fill_s": tf, "flats_s": tz, "flats_seam_iters": seam_iters, "fa_d8_s": ta, "fa_dinf_s": ti,
-                "fill_exchange_rounds": frounds, "fa_d8_rounds": arounds, "fa_dinf_rounds": irounds}
+                "fill_exchange_rounds": frounds, "fa_d8_rounds": arounds, "fa_dinf_rounds": irounds,
+                "d8_dirs_accum_s": td, "d8_dirs_seam_iters": dseam, "d8_accum_rounds": drounds}
         print(json.dumps(case), flush=True)
         res["cases"].append(case)
 if rank == 0:
