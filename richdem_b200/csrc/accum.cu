@@ -1595,13 +1595,14 @@ __global__ void __launch_bounds__(256) band_apply_packed_kernel(unsigned long lo
 // tiles; the cells on a tile's edge are its *slots*.  Almost every D8 path is short, so almost all the work stays in
 // shared memory and only the flow that crosses tile edges goes through a small global solve:
 //   1. fa_tile_codes_kernel: per tile, the flow codes from the DEM window (tile + one-cell apron) -> code bytes
-//      (tile-major scratch), then the in-tile accumulation of unit flow.  Per slot it records in `link`: for an
-//      *exit* slot (receiver in another tile) the receiver's slot, for any other slot the exit slot of the same tile
-//      where its in-tile path leaves the tile (or none), and in `lword` the exit slot's local accumulation.
+//      (tile-major scratch), then every cell's root (the last in-tile cell on its path) by pointer jumping.  Per slot
+//      it records in `link`: for an *exit* slot (receiver in another tile) the receiver's slot, for any other slot the
+//      exit slot of the same tile where its in-tile path leaves the tile (or none), and in `lword` the exit slot's
+//      local accumulation, the number of the tile's data cells whose root it is.
 //   2. fa_link_count_kernel + fa_link_walk_kernel: exit slot p drains into next(p), the exit slot where the in-tile
 //      path from its receiver's slot leaves that tile.  The exit slots form a forest, solved by the packed countdown
 //      walk over slots; each exit's total outflow is added to the inflow of its receiver's slot.
-//   3. fa_tile_final_kernel: per tile, the codes again, every cell seeded with 1 plus the inflow on its slot, the same
+//   3. fa_tile_final_kernel: per tile, the codes again, every cell seeded with 1 plus the inflow on its slot, the
 //      in-tile accumulation, the result written as doubles.
 // Per cell, HBM sees 4 B (DEM) + 2 x 1 B (codes) + 8 B (result); per slot (1/16 of the cells) 16 B of link data.  No
 // global atomic touches the cell raster.  All sums are integers < 2^31, so the result is exact whatever the order.
@@ -1689,22 +1690,28 @@ __device__ __forceinline__ void fa_tile_accumulate(const uint8_t *sCode, unsigne
   __syncthreads();
 }
 
+// Flags of a root in fa_tile_codes_kernel's parent array (cell indices need 12 bits): the path leaves the tile here, or it
+// ends here (no receiver, or NoData).
+constexpr int kFaRootExit = 0x8000, kFaRootEnd = 0x4000;
+
+// Pass 1 needs no accumulation.  Per slot the link solve needs the exit slot where its in-tile path leaves the tile, and
+// per exit slot the number of the tile's data cells whose in-tile path ends there.  Both follow from each cell's *root*,
+// the last in-tile cell on its path, which pointer jumping finds in at most ceil(log2 4096) = 12 rounds of shared-memory
+// loads; a walk would take as many dependent steps as the tile's longest in-tile path.
 __global__ void __launch_bounds__(256) fa_tile_codes_kernel(const float *__restrict__ dem, uint8_t *__restrict__ code,
                                                              int *__restrict__ link, unsigned long long *__restrict__ lword,
                                                              unsigned *__restrict__ inflow, int W, int H, float nodata,
                                                              int tiles_x) {
   constexpr int kWin = kFaT + 2;  // DEM window: the tile and a one-cell apron
-  static_assert(kWin * kWin * sizeof(float) <= kFaCells * sizeof(unsigned long long), "the DEM window lives in sWord");
-  __shared__ __align__(16) unsigned long long sWord[kFaCells];  // first the DEM window, then the accumulation words
+  static_assert(kFaCells * sizeof(uint16_t) <= kWin * kWin * sizeof(float), "the parent array lives in the DEM window");
+  __shared__ __align__(16) float sDem[kWin * kWin];  // first the DEM window, then the parent array
   __shared__ __align__(16) uint8_t sCode[kFaCells];
-  __shared__ uint16_t sQueue[kFaCells];
-  __shared__ int sCount[2];
+  __shared__ unsigned sCount[kFaSlots];  // per exit slot: the data cells whose in-tile path ends there
   const int t = threadIdx.x, tile = blockIdx.x;
-  if (t < 2) sCount[t] = 0;
+  sCount[t] = 0;
   const int bx = tile % tiles_x, by = tile / tiles_x;
   const int x0 = bx * kFaT, y0 = by * kFaT;
   const int tw = fa_side(W - x0), th = fa_side(H - y0);
-  float *sDem = reinterpret_cast<float *>(sWord);
   for (int i = t; i < kWin * kWin; i += 256) {
     const int wy = i / kWin, wx = i - wy * kWin;
     const int gy = y0 - 1 + wy, gx = x0 - 1 + wx;
@@ -1752,32 +1759,60 @@ __global__ void __launch_bounds__(256) fa_tile_codes_kernel(const float *__restr
   }
   __syncthreads();  // the DEM window is dead from here on
   reinterpret_cast<uint4 *>(code + (size_t)tile * kFaCells)[t] = reinterpret_cast<const uint4 *>(sCode)[t];
-  for (int c = t; c < kFaCells; c += 256) sWord[c] = 1;
-  fa_tile_accumulate(sCode, sWord, sQueue, sCount, tw, th);
+  // parents: a cell's in-tile receiver; a root holds its own index and its flag.  Bit k of `live`: cell t + 256 k has no
+  // root yet.
+  uint16_t *sPar = reinterpret_cast<uint16_t *>(sDem);
+  unsigned live = 0;
+#pragma unroll
+  for (int k = 0; k < kFaCells / 256; k++) {
+    const int c = t + 256 * k, cd = sCode[c], d = cd & 15;
+    int p = c | kFaRootEnd;
+    if (cd != kCodeNoData && d != 0) {
+      const int x = (c & (kFaT - 1)) + d8dx(d), y = c / kFaT + d8dy(d);
+      if (x < 0 || y < 0 || x >= tw || y >= th) {
+        p = c | kFaRootExit;
+      } else {
+        p = y * kFaT + x;
+        live |= 1u << k;
+      }
+    }
+    sPar[c] = (uint16_t)p;
+  }
+  // Pointer jumping, p[c] = p[p[c]], until every cell holds its flagged root.  Only the owner writes a cell's entry, and
+  // every value anyone reads is an ancestor on the path (a newer one is further up), so the barrier per round is all the
+  // ordering needed; it bounds the rounds by the log of the longest in-tile path.  Paths descend, so there are no cycles.
+  while (__syncthreads_or(live)) {
+#pragma unroll
+    for (int k = 0; k < kFaCells / 256; k++) {
+      if (live >> k & 1) {
+        const int c = t + 256 * k, q = sPar[sPar[c]];
+        sPar[c] = (uint16_t)q;
+        if (q & (kFaRootExit | kFaRootEnd)) live &= ~(1u << k);
+      }
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < kFaCells / 256; k++) {
+    const int r = sPar[t + 256 * k];
+    if (r & kFaRootExit) atomicAdd(&sCount[fa_slot_of(r & (kFaT - 1), (r & (kFaCells - 1)) / kFaT, tw, th)], 1u);
+  }
+  __syncthreads();
   // ---- per slot (one per thread): where its in-tile path leaves the tile ----
   const size_t gs = (size_t)tile * kFaSlots + t;
   int lk = -1;  // -1: the path ends inside the tile (or the slot is NoData / unused)
   unsigned long long out = 0;
   int lx, ly;
-  if (fa_slot_cell(t, tw, th, lx, ly) && sCode[ly * kFaT + lx] != kCodeNoData) {
-    int cur = ly * kFaT + lx;
-    for (;;) {
-      const int d = sCode[cur] & 15;
-      if (d == 0) break;
-      const int cx = cur & (kFaT - 1), cy = cur / kFaT;
-      const int x = cx + d8dx(d), y = cy + d8dy(d);
-      if (x < 0 || y < 0 || x >= tw || y >= th) {
-        if (cur == ly * kFaT + lx) {  // an exit slot: link to the receiver's slot (encoded as -2 - slot)
-          const int gx = x0 + x, gy = y0 + y, rbx = gx / kFaT, rby = gy / kFaT;
-          const int rs = fa_slot_of(gx - rbx * kFaT, gy - rby * kFaT, fa_side(W - rbx * kFaT), fa_side(H - rby * kFaT));
-          lk = -2 - ((rby * tiles_x + rbx) * kFaSlots + rs);
-          out = kLkOne | (sWord[cur] & kPkVal);  // the count starts at 1: the slot's own token (fa_link_walk_kernel)
-        } else {
-          lk = tile * kFaSlots + fa_slot_of(cx, cy, tw, th);
-        }
-        break;
-      }
-      cur = y * kFaT + x;
+  if (fa_slot_cell(t, tw, th, lx, ly)) {
+    const int c = ly * kFaT + lx, r = sPar[c];
+    if (r == (c | kFaRootExit)) {  // an exit slot: link to the receiver's slot (encoded as -2 - slot)
+      const int d = sCode[c] & 15;
+      const int gx = x0 + lx + d8dx(d), gy = y0 + ly + d8dy(d), rbx = gx / kFaT, rby = gy / kFaT;
+      const int rs = fa_slot_of(gx - rbx * kFaT, gy - rby * kFaT, fa_side(W - rbx * kFaT), fa_side(H - rby * kFaT));
+      lk = -2 - ((rby * tiles_x + rbx) * kFaSlots + rs);
+      out = kLkOne | sCount[t];  // the count starts at 1: the slot's own token (fa_link_walk_kernel)
+    } else if (r & kFaRootExit) {
+      const int e = r & (kFaCells - 1);
+      lk = tile * kFaSlots + fa_slot_of(e & (kFaT - 1), e / kFaT, tw, th);
     }
   }
   link[gs] = lk;
