@@ -250,6 +250,7 @@ int rdb200_set_param(const char *name, int64_t value) {
   else if (n == "fill_max_iters") p.fill_max_iters = value;
   else if (n == "fill_rounds_per_sync") p.fill_rounds_per_sync = value > 0 ? value : 16;
   else if (n == "fill_use_tma") p.fill_use_tma = value;
+  else if (n == "fill_external_z") p.fill_external_z = value;
   else if (n == "fill_profile") p.fill_profile = value;
   else if (n == "fill_trace") p.fill_trace = value;
   else if (n == "fill_ordered") p.fill_ordered = value;

@@ -83,7 +83,15 @@ struct FillDev {
 };
 
 struct FillArgs {
-  const float *Zp;
+  // Z of cell (x, y) is Z[(y + zoy) * zpitch + x + zox]: the padded copy (pitch, 1, PADL), or the caller's w x h raster
+  // itself (zext: row stride W, no offsets; cells outside the raster read as +inf)
+  const float *Z;
+  int zpitch, zox, zoy, zext;
+  // round 1 of a lifted start: W is built from the coarse surface instead of loaded (null: load it); `staged` flags the
+  // tiles whose cells are in Wp already
+  const float *coarse;
+  int Wc, pool, yoff;
+  int *staged;
   float *Wp;
   int pitch;  // floats
   int W, H;
@@ -188,7 +196,9 @@ __device__ __forceinline__ float min3f(float a, float b, float c) { return fminf
 // STEP = 1: geodesic distance,      new = min(W, max(Z, 1 + min8 W))   with Z = 0 on cells the flood
 //           may enter and +inf elsewhere (used for the flat-resolution gradients, csrc/flats.cu)
 // TOPO4: the 4-neighbour (D4) stencil of FillDepressions<Topology::D4>; corner aprons are then never read
-template <int STEP, bool TOPO4 = false>
+// STAGE: round 1 of a staged lifted start (a.coarse): W is built from the coarse surface, not loaded, and every row is
+//        written back (a template parameter so that the later rounds keep their registers)
+template <int STEP, bool TOPO4 = false, bool STAGE = false>
 __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
     fill_sweep_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__ CUtensorMap mapZ,
                       const FillArgs a) {
@@ -204,6 +214,7 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
   __shared__ int sFlags;
   __shared__ int sKey;
   __shared__ int sProf[2];
+  __shared__ int sNbDone;  // staged round: neighbours (bit (dy + 1) * 3 + dx + 1) whose cells are in Wp already
 
   const int tid = threadIdx.x;
   const int r = a.round;
@@ -250,36 +261,89 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
     const int x0 = txT * TX, y0 = tyT * TY;  // raster coords of the tile's first cell
 
     // ---- stage W (+apron) and Z ----
+    constexpr bool stage = STAGE;
     if (tid == 0) {
       sFlags = 0;
       sKey = ORD_POS_INF;
       sProf[0] = sProf[1] = 0;
+      if (stage) {
+        // neighbours visited earlier in this round have written their cells, and a load of the window would see them
+        int nb = 0;
+        for (int dy = -1; dy <= 1; dy++)
+          for (int dx = -1; dx <= 1; dx++) {
+            const int ty = tyT + dy, tx = txT + dx;
+            if ((dx | dy) && ty >= 0 && ty < a.tilesY && tx >= 0 && tx < a.tilesX &&
+                *reinterpret_cast<volatile int *>(&a.staged[ty * a.tilesX + tx]))
+              nb |= 1 << ((dy + 1) * 3 + dx + 1);
+          }
+        __threadfence();  // their Wp stores are read after their flags
+        sNbDone = nb;
+      }
     }
     if (a.use_tma) {
       if (tid == 0) {
         fence_proxy_async();  // order earlier generic-proxy smem accesses before the async writes
-        mbar_arrive_expect_tx(&mbar, W_TILE_BYTES + Z_TILE_BYTES);
-        tma_load_2d(sW, &mapW, x0, y0, &mbar);               // padded cols x0..x0+71, rows y0..y0+65
-        tma_load_2d(sZ, &mapZ, x0 + PADL, y0 + 1, &mbar);    // the 64x64 interior
+        mbar_arrive_expect_tx(&mbar, (stage ? 0u : W_TILE_BYTES) + Z_TILE_BYTES);
+        if (!stage) tma_load_2d(sW, &mapW, x0, y0, &mbar);  // padded cols x0..x0+71, rows y0..y0+65
+        tma_load_2d(sZ, &mapZ, x0 + a.zox, y0 + a.zoy, &mbar);  // the 64x64 interior
       }
     } else {
-      for (int k = tid; k < SROWS * (SP / 4); k += FILL_THREADS) {
-        const int rr = k / (SP / 4), cc = k - rr * (SP / 4);
-        reinterpret_cast<float4 *>(sW)[k] =
-            __ldcg(reinterpret_cast<const float4 *>(a.Wp + (size_t)(y0 + rr) * a.pitch + x0) + cc);
+      if (!stage) {
+        for (int k = tid; k < SROWS * (SP / 4); k += FILL_THREADS) {
+          const int rr = k / (SP / 4), cc = k - rr * (SP / 4);
+          reinterpret_cast<float4 *>(sW)[k] =
+              __ldcg(reinterpret_cast<const float4 *>(a.Wp + (size_t)(y0 + rr) * a.pitch + x0) + cc);
+        }
       }
+      const float inf = __int_as_float(0x7f800000);
       for (int k = tid; k < TY * (TX / 4); k += FILL_THREADS) {
         const int rr = k / (TX / 4), cc = k - rr * (TX / 4);
-        reinterpret_cast<float4 *>(sZ)[k] = __ldg(
-            reinterpret_cast<const float4 *>(a.Zp + (size_t)(y0 + 1 + rr) * a.pitch + x0 + PADL) + cc);
+        // (W % 4 == 0 in zext mode: a float4 lies wholly inside or wholly outside the raster)
+        reinterpret_cast<float4 *>(sZ)[k] =
+            a.zext && (y0 + rr >= a.H || x0 + 4 * cc >= a.W)
+                ? make_float4(inf, inf, inf, inf)
+                : __ldg(reinterpret_cast<const float4 *>(a.Z + (size_t)(y0 + a.zoy + rr) * a.zpitch + x0 + a.zox) + cc);
       }
     }
     // ---- initial dirty list from the apron sides that changed (overlaps the TMA flight) ----
     int sides = a.sides[(r & 1) * ntiles + t];
-    __syncthreads();  // everyone has read `sides` before it is cleared
+    __syncthreads();  // everyone has read `sides` before it is cleared (and sees sNbDone)
     if (tid == 0) {
       a.sides[(r & 1) * ntiles + t] = 0;
       a.keys[(r & 1) * ntiles + t] = ORD_POS_INF;
+    }
+    if (stage) {
+      // The start W0 of fill_init_kernel<true>, built here instead of loaded: Z on the raster border, +inf outside the
+      // raster, elsewhere the coarse level of the cell's pool x pool block.  Apron cells of a neighbour that is done
+      // with this round come from Wp.
+      const float inf = __int_as_float(0x7f800000);
+      const int nbdone = sNbDone;
+      for (int k = tid; k < SROWS * (SP / 4); k += FILL_THREADS) {
+        const int rr = k / (SP / 4), c4 = 4 * (k - rr * (SP / 4));
+        const int dy = rr == 0 ? -1 : (rr == SROWS - 1 ? 1 : 0), dx = c4 < PADL ? -1 : (c4 >= PADL + TX ? 1 : 0);
+        float4 v4;
+        if ((nbdone >> ((dy + 1) * 3 + dx + 1)) & 1) {
+          v4 = __ldcg(reinterpret_cast<const float4 *>(a.Wp + (size_t)(y0 + rr) * a.pitch + x0 + c4));
+        } else {
+          const int y = y0 + rr - 1, xb = x0 + c4 - PADL;  // raster coords of the first of the 4 cells
+          float v[4] = {inf, inf, inf, inf};
+          if (y >= 0 && y < a.H) {
+            const float *crow = a.coarse + (size_t)((y + a.yoff) / a.pool) * a.Wc;
+            const float *zrow = a.Z + (size_t)(y + a.zoy) * a.zpitch + a.zox;
+            const bool brow = y == 0 || y == a.H - 1;
+            // xb is a multiple of 4: with pool % 4 == 0 the 4 cells share one coarse block
+            const float c0 = (a.pool & 3) == 0 && xb >= 0 && xb < a.W ? __ldg(crow + xb / a.pool) : inf;
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+              const int x = xb + j;
+              if (x >= 0 && x < a.W)
+                v[j] = brow || x == 0 || x == a.W - 1 ? __ldg(zrow + x) : (a.pool & 3) == 0 ? c0 : __ldg(crow + x / a.pool);
+            }
+          }
+          v4 = make_float4(v[0], v[1], v[2], v[3]);
+        }
+        *reinterpret_cast<float4 *>(&sW[rr * SP + c4]) = v4;
+      }
     }
 #include "fill_relax_body.inc"
 
@@ -291,15 +355,26 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
     __syncthreads();
     const int fl = sFlags;
     const int rowch = (fl >> 12) & 0xFFFF;
-    if (rowch) {
+    // a staged round writes every row: it is what initialises the tile's cells in Wp
+    const int rowout = stage ? (1 << BYN) - 1 : rowch;
+    if (rowout) {
       // coalesced float4 write-back of the block rows (4 cell rows x 64) that hold a change
       for (int k = tid; k < TY * (TX / 4); k += FILL_THREADS) {
         const int rr = k / (TX / 4), cc = k % (TX / 4);
-        if (rowch & (1 << (rr >> 2))) {
+        if (rowout & (1 << (rr >> 2))) {
           const float4 val = *reinterpret_cast<const float4 *>(&sW[(rr + 1) * SP + PADL + 4 * cc]);
           __stcg(reinterpret_cast<float4 *>(a.Wp + (size_t)(y0 + 1 + rr) * a.pitch + (x0 + PADL)) + cc, val);
         }
       }
+    }
+    if (stage) {
+      __syncthreads();  // every cell of the tile is stored ...
+      if (tid == 0) {
+        __threadfence();  // ... and visible to the GPU before the flag
+        atomicExch(&a.staged[t], 1);
+      }
+    }
+    if (rowch) {
       if (tid < 8) {
         // one thread per neighbour: the enqueue atomics (or + exch + add) overlap instead of
         // queueing behind each other on a single thread
@@ -428,6 +503,7 @@ __global__ void __launch_bounds__(256) fill_lift_row_kernel(float *row, int W, c
 // are boundary conditions: W = Z = dem there; interior W = +inf; padding Z = W = +inf.
 // LIFT (fill_multigrid): interior cells start at the water level of their pool x pool block in the filled max-pooled
 // raster `coarse` (an upper bound of the answer, see fill_depressions_dev) instead of +inf.
+// Zp may be null: the sweep then reads Z from `dem` itself.
 template <bool LIFT>
 __global__ void fill_init_kernel(const float *__restrict__ dem, float *__restrict__ Zp,
                                  float *__restrict__ Wp, int W, int H, int pitch, int rows, FillDev *dev,
@@ -455,7 +531,7 @@ __global__ void fill_init_kernel(const float *__restrict__ dem, float *__restric
       wv[k] = ww;
     }
     const size_t o = (size_t)py * pitch + px4;
-    *reinterpret_cast<float4 *>(Zp + o) = make_float4(zv[0], zv[1], zv[2], zv[3]);
+    if (Zp) *reinterpret_cast<float4 *>(Zp + o) = make_float4(zv[0], zv[1], zv[2], zv[3]);
     *reinterpret_cast<float4 *>(Wp + o) = make_float4(wv[0], wv[1], wv[2], wv[3]);
   }
   for (int o = 16; o > 0; o >>= 1) {
@@ -478,17 +554,36 @@ __global__ void fill_init_kernel(const float *__restrict__ dem, float *__restric
   }
 }
 
-// sampled histogram of the input elevations (every `row_stride`-th padded row) for the level schedule
+// padded W of a staged lifted start: only the padding frame (rows 0 and rows - 1, PADL columns on either side) is +inf
+// here; the first sweep round writes every tile's cells
+__global__ void __launch_bounds__(256) fill_frame_kernel(float *__restrict__ Wp, int pitch, int rows) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const float inf = __int_as_float(0x7f800000);
+  if (i < pitch) {
+    Wp[i] = inf;
+    Wp[(size_t)(rows - 1) * pitch + i] = inf;
+  }
+  if (i < rows) {
+#pragma unroll
+    for (int j = 0; j < PADL; j++) {
+      Wp[(size_t)i * pitch + j] = inf;
+      Wp[(size_t)i * pitch + pitch - PADL + j] = inf;
+    }
+  }
+}
+
+// sampled histogram of the input elevations (every `row_stride`-th row of `ncols` x `nrows` floats, row pitch `zpitch`;
+// +inf padding is skipped) for the level schedule
 constexpr int HIST_BINS = 1024;
-__global__ void __launch_bounds__(256) fill_hist_kernel(const float *__restrict__ Zp, int pitch, int rows, int row_stride,
-                                                         float zmin, float inv_range, unsigned int *hist) {
+__global__ void __launch_bounds__(256) fill_hist_kernel(const float *__restrict__ Z, int zpitch, int ncols, int nrows,
+                                                         int row_stride, float zmin, float inv_range, unsigned int *hist) {
   __shared__ unsigned int sh[HIST_BINS];
   for (int k = threadIdx.x; k < HIST_BINS; k += blockDim.x) sh[k] = 0;
   __syncthreads();
-  const int row = blockIdx.x * row_stride + 1;
-  if (row < rows) {
-    for (int x = threadIdx.x; x < pitch; x += blockDim.x) {
-      const float zv = Zp[(size_t)row * pitch + x];
+  const int row = blockIdx.x * row_stride;
+  if (row < nrows) {
+    for (int x = threadIdx.x; x < ncols; x += blockDim.x) {
+      const float zv = Z[(size_t)row * zpitch + x];
       if (zv < __int_as_float(0x7f800000) && zv > -__int_as_float(0x7f800000)) {
         int b = (int)((zv - zmin) * inv_range * HIST_BINS);
         b = b < 0 ? 0 : (b >= HIST_BINS ? HIST_BINS - 1 : b);
@@ -780,6 +875,7 @@ struct FillState {
   DevBuf<float> Zp, Wp;
   DevBuf<int> list0, list1, plist, stamp, sides, keys;
   DevBuf<int> dirty, tflag;  // V-cycle bookkeeping: tiles written since the last look / tiles to wake (both per tile)
+  DevBuf<int> staged;        // staged lifted start: tiles the first round has written (per tile)
   float zmin = 0.f, zmax = 0.f;
   bool first_run = true;
   bool ordered = false;
@@ -796,8 +892,17 @@ struct FillState {
   bool still_active = false;
   int64_t sched_round = 0;
 
+  // Z read straight from the caller's raster (no padded copy; see begin's `dem_stays`)
+  const float *zext = nullptr;
+  // staged lifted start: the first sweep round builds W from this coarse surface (see fill_sweep_kernel)
+  const float *stage_coarse = nullptr;
+  int stage_wc = 0, stage_k = 1, stage_yoff = 0;
+
+  // dem_stays: d_dem is left as it is until finish() (and the state uses no row updates), so the sweep may read Z from
+  // it instead of a padded copy.  It does so when TMA can address the raster: width a multiple of 4, 16-byte aligned.
+  // With a lifted start, that also lets the first round build its W from the coarse surface (no W pass beforehand).
   void begin(const float *d_dem, int w, int h, const float *d_coarse = nullptr, int coarse_w = 0, int coarse_k = 0,
-             int coarse_yoff = 0) {
+             int coarse_yoff = 0, bool dem_stays = false) {
     Ctx &c = ctx();
     W = w;
     H = h;
@@ -806,7 +911,13 @@ struct FillState {
     pitch = tilesX * TX + 2 * PADL;
     rows = tilesY * TY + 2;
     const size_t np = (size_t)pitch * rows;
-    Zp.alloc(np);
+    zext = dem_stays && c.params.fill_external_z != 0 && (w & 3) == 0 && ((uintptr_t)d_dem & 15) == 0 ? d_dem : nullptr;
+    stage_coarse = zext && d_coarse ? d_coarse : nullptr;
+    stage_wc = coarse_w;
+    stage_k = coarse_k;
+    stage_yoff = coarse_yoff;
+    if (zext) Zp.reset();
+    else Zp.alloc(np);
     Wp.alloc(np);
     const size_t nt = (size_t)tilesX * tilesY;
     list0.alloc(nt);
@@ -818,6 +929,10 @@ struct FillState {
     dev.alloc(1);
     RDB_CK(cudaMemsetAsync(stamp.p, 0, nt * sizeof(int), c.stream));
     RDB_CK(cudaMemsetAsync(sides.p, 0, 2 * nt * sizeof(int), c.stream));
+    if (stage_coarse) {
+      staged.alloc(nt);
+      RDB_CK(cudaMemsetAsync(staged.p, 0, nt * sizeof(int), c.stream));
+    }
     {
       FillDev h0;
       memset(&h0, 0, sizeof(h0));
@@ -832,19 +947,28 @@ struct FillState {
       const int n2 = (int)(2 * nt);
       fill_i32_kernel<<<(n2 + 255) / 256, 256, 0, c.stream>>>(keys.p, ORD_POS_INF, n2);
       dim3 blk(128), grd((pitch / 4 + 127) / 128, rows < 2048 ? rows : 2048);
-      if (d_coarse)
+      if (stage_coarse) {
+        // the first round writes every tile's cells; only the frame is left (zmin / zmax serve the level schedule,
+        // which a lifted start does not use)
+        const int n = pitch > rows ? pitch : rows;
+        fill_frame_kernel<<<(n + 255) / 256, 256, 0, c.stream>>>(Wp.p, pitch, rows);
+      } else if (d_coarse) {
         fill_init_kernel<true><<<grd, blk, 0, c.stream>>>(d_dem, Zp.p, Wp.p, W, H, pitch, rows, dev.p, d_coarse, coarse_w, coarse_k,
                                                          coarse_yoff);
-      else
+      } else {
         fill_init_kernel<false><<<grd, blk, 0, c.stream>>>(d_dem, Zp.p, Wp.p, W, H, pitch, rows, dev.p, nullptr, 0, 1, 0);
+      }
       RDB_CK(cudaGetLastError());
       count_launch(2);
-      FillDev *hd = (FillDev *)c.pinned;
-      RDB_CK(cudaMemcpyAsync(hd, dev.p, sizeof(FillDev), cudaMemcpyDeviceToHost, c.stream));
-      RDB_CK(cudaStreamSynchronize(c.stream));
-      zmin = ord2f(hd->zmin_ord);
-      zmax = ord2f(hd->zmax_ord);
-      if (!(zmin <= zmax)) zmin = zmax = 0.f;
+      zmin = zmax = 0.f;
+      if (!d_coarse) {
+        FillDev *hd = (FillDev *)c.pinned;
+        RDB_CK(cudaMemcpyAsync(hd, dev.p, sizeof(FillDev), cudaMemcpyDeviceToHost, c.stream));
+        RDB_CK(cudaStreamSynchronize(c.stream));
+        zmin = ord2f(hd->zmin_ord);
+        zmax = ord2f(hd->zmax_ord);
+        if (!(zmin <= zmax)) zmin = zmax = 0.f;
+      }
       // a lifted start (fill_multigrid) is already close to the answer everywhere: no level schedule
       ordered = c.params.fill_ordered != 0 && zmax > zmin && !d_coarse;
       levels.clear();
@@ -860,7 +984,12 @@ struct FillState {
           RDB_CK(cudaMemsetAsync(hist.p, 0, HIST_BINS * sizeof(unsigned int), c.stream));
           const int stride = rows > 4096 ? 16 : (rows > 512 ? 4 : 1);
           const int nb = (rows - 2 + stride - 1) / stride;
-          fill_hist_kernel<<<nb, 256, 0, c.stream>>>(Zp.p, pitch, rows, stride, zmin, 1.0f / (zmax - zmin), hist.p);
+          // (padded rows 1, 1 + stride, ... are raster rows 0, stride, ...)
+          if (zext)
+            fill_hist_kernel<<<nb, 256, 0, c.stream>>>(zext, W, W, H, stride, zmin, 1.0f / (zmax - zmin), hist.p);
+          else
+            fill_hist_kernel<<<nb, 256, 0, c.stream>>>(Zp.p + pitch, pitch, pitch, rows - 1, stride, zmin, 1.0f / (zmax - zmin),
+                                                       hist.p);
           RDB_CK(cudaGetLastError());
           count_launch();
           unsigned int *hh = (unsigned int *)c.pinned;
@@ -880,7 +1009,8 @@ struct FillState {
       }
     }
     mapW = make_map(Wp.p, pitch, rows, SP, SROWS);
-    mapZ = make_map(Zp.p, pitch, rows, TX, TY);
+    // (TMA fills the box cells beyond the raster's edge with zeros; the sweep overwrites them with +inf)
+    mapZ = zext ? make_map(const_cast<float *>(zext), W, H, TX, TY) : make_map(Zp.p, pitch, rows, TX, TY);
     int per_sm = 0;
     RDB_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fill_sweep_kernel<0>, FILL_THREADS, 0));
     if (per_sm < 1) per_sm = 1;
@@ -959,7 +1089,20 @@ struct FillState {
     Ctx &c = ctx();
     FillArgs a;
     memset(&a, 0, sizeof(a));
-    a.Zp = Zp.p;
+    if (zext) {
+      a.Z = zext;
+      a.zpitch = W;
+      a.zext = 1;
+    } else {
+      a.Z = Zp.p;
+      a.zpitch = pitch;
+      a.zox = PADL;
+      a.zoy = 1;
+    }
+    a.Wc = stage_wc;
+    a.pool = stage_k;
+    a.yoff = stage_yoff;
+    a.staged = staged.p;
     a.Wp = Wp.p;
     a.pitch = pitch;
     a.W = W;
@@ -1002,7 +1145,11 @@ struct FillState {
         a.use_proc = 0;
       }
       sched_round++;
+      // round 1 of a staged lifted start visits every tile (seeded in begin) and builds W instead of loading it
+      a.coarse = round == 1 ? stage_coarse : nullptr;
       if (step_mode) fill_sweep_kernel<1><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mapZ, a);
+      else if (a.coarse && topo4) fill_sweep_kernel<0, true, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mapZ, a);
+      else if (a.coarse) fill_sweep_kernel<0, false, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mapZ, a);
       else if (topo4) fill_sweep_kernel<0, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mapZ, a);
       else fill_sweep_kernel<0><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mapZ, a);
       round++;
@@ -1316,7 +1463,8 @@ static void fill_depressions_level(float *d_dem, int w, int h, int depth, bool t
     extra.fill_rounds -= before.fill_rounds;
     extra.fill_tile_visits -= before.fill_tile_visits;
     extra.fill_tile_iters -= before.fill_tile_iters;
-    st.begin(d_dem, w, h, coarse.p, wc, k);
+    // (d_dem, zc and coarse stay as they are until st.finish: the solvers read Z, and round 1 its start, from them)
+    st.begin(d_dem, w, h, coarse.p, wc, k, 0, true);
     if (every <= 0) {
       st.run();
     } else {
@@ -1331,7 +1479,7 @@ static void fill_depressions_level(float *d_dem, int w, int h, int depth, bool t
       // looks at the fine tiles below those -- a correction costs what it changes, not three passes over the raster.
       FillState cst;
       cst.topo4 = topo4;
-      cst.begin(zc.p, wc, hc, coarse.p, wc, 1);  // start: the coarse fill itself (already a fixed point)
+      cst.begin(zc.p, wc, hc, coarse.p, wc, 1, 0, true);  // start: the coarse fill itself (already a fixed point)
       cst.run();                                  // (drains the initial all-tiles worklist; nothing moves)
       cst.track_dirty();
       st.track_dirty();
@@ -1383,7 +1531,7 @@ static void fill_depressions_level(float *d_dem, int w, int h, int depth, bool t
     return;
   }
   if (w <= 2 || h <= 2) return;  // every cell is a border cell: nothing can change
-  st.begin(d_dem, w, h);
+  st.begin(d_dem, w, h, nullptr, 0, 0, 0, true);
   st.run();
   st.finish(d_dem);
   RDB_CK(cudaStreamSynchronize(c.stream));
