@@ -322,6 +322,7 @@ __global__ void __launch_bounds__(256) accum_walk_kernel(const WalkArgs<A> a) {
         // I am the receiver's only donor: no other thread touches accum[r] before I hand it on
         const A sum = ld_acc(a.accum + r) + acc;
         a.accum[r] = sum;
+        if (CHECK) a.st[r] = 0;  // released: after the walk, donors left in st mark a direction grid's unreleased cells
         acc = sum;
         c = r;
         continue;
@@ -597,6 +598,14 @@ void run_walk(WalkArgs<A> a, size_t ncells) {
 __global__ void area_init_kernel(const uint8_t *__restrict__ dirs, int32_t *__restrict__ area, size_t n) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) area[i] = (dirs[i] == kCodeNoData) ? -1 : 1;  // d8_methods.hpp:71-74, :111
+}
+
+// A direction grid may hold loops.  A cell on a loop, or downstream of one, keeps donors that never complete; the
+// reference never takes it off its source queue, so it never adds its own unit (d8_methods.hpp:105-111) and keeps only
+// the inflow it received.  After the walk such a cell still has donors left in st: it gives back the 1 of area_init.
+__global__ void area_unreleased_kernel(const uint32_t *__restrict__ st, int32_t *__restrict__ area, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && (st[i] & kDepsMask) != 0) area[i] -= 1;
 }
 
 __global__ void sanitize_dirs_kernel(const uint8_t *__restrict__ dirs, uint8_t *__restrict__ code, size_t n) {
@@ -2055,6 +2064,9 @@ void d8_flow_accum_dev(const uint8_t *d_dirs, int32_t *d_area, int w, int h) {
   a.W = w;
   a.H = h;
   run_walk<0, true, int32_t>(a, n);
+  area_unreleased_kernel<<<blocks, 256, 0, c.stream>>>(st.p, d_area, n);
+  RDB_CK(cudaGetLastError());
+  count_launch();
 }
 
 }  // namespace rdb
@@ -2169,15 +2181,21 @@ __global__ void __launch_bounds__(256) band_settle_dir_codes_kernel(uint8_t *cod
   if (nx < 0 || ny < 0 || nx >= W || ny >= H || code[(size_t)ny * W + nx] == kCodeNoData) code[i] = 0;
 }
 
-// the int32 areas from the accumulator: doubles, or -- packed words of cells that never completed, which only a cycle
-// in the direction grid leaves behind -- [donors left (1..8) | integer sum], the partial sum d8_flow_accum leaves there
+// the int32 areas from the accumulator: doubles, or -- packed words of cells that never completed, which only a loop in
+// the direction grid leaves behind -- [donors left (1..8) | integer sum].  Such an unreleased cell (on a loop or
+// downstream of one; unpacked: donors left in st) keeps only the inflow it received, without its own unit, as in
+// d8_flow_accum (area_unreleased_kernel).
 __global__ void __launch_bounds__(256) band_area_from_accum_kernel(const unsigned long long *__restrict__ word,
+                                                                    const uint32_t *__restrict__ st,
                                                                     int32_t *__restrict__ area, size_t n, int packed) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const unsigned long long v = word[i];
   const unsigned top = (unsigned)(v >> 56);
-  area[i] = (packed && top >= 1 && top <= 8) ? (int32_t)(v & kPkVal) : (int32_t)__longlong_as_double((long long)v);
+  if (packed)
+    area[i] = (top >= 1 && top <= 8) ? (int32_t)(v & kPkVal) - 1 : (int32_t)__longlong_as_double((long long)v);
+  else
+    area[i] = (int32_t)__longlong_as_double((long long)v) - ((st[i] & kDepsMask) != 0 ? 1 : 0);
 }
 
 }  // namespace
@@ -2381,7 +2399,9 @@ struct FaccState {
     for (;;) {
       const unsigned blocks = (unsigned)(((size_t)a.nfrontier + 255) / 256);
       if (blocks) {
-        accum_walk_kernel<MODE, false, double, true><<<blocks, 256, 0, c.stream>>>(a);
+        // a direction grid walks with CHECK (the sole-donor steps clear st, which tells unreleased cells at the end)
+        if (from_dirs) accum_walk_kernel<MODE, true, double, true><<<blocks, 256, 0, c.stream>>>(a);
+        else accum_walk_kernel<MODE, false, double, true><<<blocks, 256, 0, c.stream>>>(a);
         RDB_CK(cudaGetLastError());
         count_launch();
       }
@@ -2747,7 +2767,7 @@ void mgpu_d8_flow_accum_band(const rdb200_comm *comm, const uint8_t *d_dirs, int
     A.begin_dirs(d_dirs, acc.p, w, hloc, gt, gb);
     fa_band_rounds(comm, A, xrounds);
     band_area_from_accum_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(
-        reinterpret_cast<const unsigned long long *>(acc.p), d_area, n, A.packed ? 1 : 0);
+        reinterpret_cast<const unsigned long long *>(acc.p), A.st.p, d_area, n, A.packed ? 1 : 0);
     RDB_CK(cudaGetLastError());
     count_launch();
   }
