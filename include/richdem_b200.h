@@ -249,7 +249,7 @@ RDB200_API int rdb200_dev_generate_fbm_f32(float *d_dem, int32_t width, int32_t 
  *
  *   rank 0:  rdb200_nccl_unique_id(id)   ... ship the 128 bytes to every rank (MPI_Bcast, a file, torch.distributed) ...
  *   all:     rdb200_init(local_gpu); rdb200_comm_create_nccl(&comm, rank, world, id);
- *            rdb200_mgpu_fill_depressions_d8_f32(comm, d_band, W, rows, gt, gb, row0, H, NULL);
+ *            rdb200_mgpu_fill_depressions_d8_f32(comm, d_band, W, rows, gt, gb, row0, H, NULL);   (or ..._d4_f32)
  *            rdb200_mgpu_resolve_flats_epsilon_f32(comm, d_band, W, rows, nodata, gt, gb, NULL);
  *            rdb200_mgpu_fa_f32_f64(comm, d_band, d_accum, W, rows, nodata, gt, gb, 0, 1, NULL);
  *   or, for the direction-grid pipeline after the fill (uint8 directions and int32 upslope-cell counts):
@@ -275,6 +275,13 @@ RDB200_API int rdb200_comm_destroy(rdb200_comm *comm);
  * rows on return).  row0 = global row of local row 0, height = rows of the whole raster.  Same result as the single-GPU
  * call, bit for bit.  *exchange_rounds (optional): halo exchanges done. */
 RDB200_API int rdb200_mgpu_fill_depressions_d8_f32(const rdb200_comm *comm, float *d_band, int32_t width, int32_t local_rows,
+                                                   int32_t ghost_top, int32_t ghost_bottom, int32_t row0, int32_t height,
+                                                   int32_t *exchange_rounds);
+/* FillDepressions<D4> (include/richdem/depressions/depressions.hpp:16-17 -> PriorityFlood_Barnes2014<Topology::D4>,
+ * include/richdem/depressions/Barnes2014.hpp:230-304) over row bands: the 4-neighbour counterpart of
+ * rdb200_mgpu_fill_depressions_d8_f32, with the same arguments and band convention.  Same result as
+ * rdb200_dev_fill_depressions_d4_f32 on one GPU, bit for bit. */
+RDB200_API int rdb200_mgpu_fill_depressions_d4_f32(const rdb200_comm *comm, float *d_band, int32_t width, int32_t local_rows,
                                                    int32_t ghost_top, int32_t ghost_bottom, int32_t row0, int32_t height,
                                                    int32_t *exchange_rounds);
 /* ResolveFlatsEpsilon (include/richdem/flats/flats.hpp:21-28) over row bands, in place on the owned rows of `d_band`

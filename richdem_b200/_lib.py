@@ -82,6 +82,7 @@ SIGNATURES = {
     "rdb200_comm_create_callbacks": [C.POINTER(_vp), _i32, _i32, _vp, _vp, _vp],
     "rdb200_comm_destroy": [_vp],
     "rdb200_mgpu_fill_depressions_d8_f32": [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_mgpu_fill_depressions_d4_f32": [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
     "rdb200_mgpu_fa_f32_f64": [_vp, _vp, _vp, _i32, _i32, _f32, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
     "rdb200_mgpu_fa_method_f32_f64": [_vp, _vp, _vp, _i32, _i32, _f32, _i32, _i32, _i32, C.c_double, _i32, C.POINTER(_i32)],
     "rdb200_mgpu_resolve_flats_epsilon_f32": [_vp, _vp, _i32, _i32, _f32, _i32, _i32, C.POINTER(_i32)],

@@ -598,6 +598,19 @@ int rdb200_mgpu_fill_depressions_d8_f32(const rdb200_comm *comm, float *d_band, 
   CAPI_END
 }
 
+int rdb200_mgpu_fill_depressions_d4_f32(const rdb200_comm *comm, float *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb,
+                                        int32_t row0, int32_t height, int32_t *exchange_rounds) {
+  int xr = 0;
+  CAPI_TRY
+  if (!d_band) fail("mgpu_fill: null pointer");
+  check_dims(w, rows);
+  CallScope cs((int64_t)w * rows);
+  mgpu_fill_band(comm, d_band, w, rows, gt, gb, row0, height, &xr, true);
+  cs.done();
+  if (exchange_rounds) *exchange_rounds = xr;
+  CAPI_END
+}
+
 int rdb200_mgpu_fa_f32_f64(const rdb200_comm *comm, const float *d_dem, double *d_accum, int32_t w, int32_t rows, float nodata,
                            int32_t gt, int32_t gb, int32_t dinf, int32_t ones, int32_t *exchange_rounds) {
   int xr = 0;

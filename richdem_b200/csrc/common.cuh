@@ -163,7 +163,8 @@ void comm_exchange(const rdb200_comm *c, const void *send_up, void *recv_up, con
 void comm_allreduce(const rdb200_comm *c, void *buf, size_t count, int op);
 void check_band_args(const char *what, const rdb200_comm *comm, const void *d_band, int w, int hloc, int gt, int gb);
 void exchange_band_rows(const rdb200_comm *comm, void *d_band, size_t elem, int w, int hloc, int gt, int gb);
-void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, int gt, int gb, int row0, int H, int *xrounds);
+void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, int gt, int gb, int row0, int H, int *xrounds,
+                    bool topo4 = false);
 // method: 0 D8, 1 Tarboton, 2 D4, 3 Holmgren (xparam; Quinn = 1.0), 4 Freeman (xparam)
 void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, int w, int hloc, float nodata, int gt, int gb,
                   int method, double xparam, bool ones, int *xrounds);

@@ -1572,7 +1572,15 @@ void fill_maxpool_rows(const float *d_src, int w, int h, int yoff, float *d_coar
 // The fixed point is the single-GPU one (any admissible schedule ends at W*, DESIGN.md 3.1): when no tile is active, no
 // ghost row dropped and no correction lowered a cell on any rank, every band is at its local fixed point with ghost rows
 // equal to the neighbours' edge rows.
-void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, int gt, int gb, int row0, int H, int *xrounds) {
+// topo4: FillDepressions<D4>.  Every solver the driver creates -- the band's, the replicated coarse fill's and the V-cycle
+// coarse solver's -- takes the 4-neighbour stencil: the lifted start is an upper bound of the D4 answer only if the coarse
+// surface is the D4 fill too (blocks that touch at a corner hold no D4-adjacent cells, so a D8 coarse fill would drain a
+// block through that corner and start the band below the answer, which relaxation cannot repair).  The rest does not
+// depend on the stencil: a ghost row takes the neighbour's edge row where it is lower (min; the tiles it wakes are the
+// D8 readers, a superset of the D4 ones), a lifted ghost row is its blocks' coarse levels, block maxima and
+// prolongation (min(fine, lifted)) are cell-wise over k x k blocks, and the termination vote counts events, not cells.
+void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, int gt, int gb, int row0, int H, int *xrounds,
+                    bool topo4) {
   Ctx &c = ctx();
   const int world = comm_world(comm);
   gt = gt ? 1 : 0;
@@ -1630,7 +1638,7 @@ void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, in
     comm_allreduce(comm, zc.p, nc, RDB200_MAX_F32);
     lap0("all-reduce pooled raster");
     RDB_CK(cudaMemcpyAsync(wcoarse.p, zc.p, nc * sizeof(float), cudaMemcpyDeviceToDevice, c.stream));
-    fill_depressions_level(wcoarse.p, wc, hc, 1);  // every rank fills the small raster itself
+    fill_depressions_level(wcoarse.p, wc, hc, 1, topo4);  // every rank fills the small raster itself
     lap0("coarse fill (replicated)");
     for (int side = 0; side < 2; side++) {
       if (!(side == 0 ? gt : gb)) continue;
@@ -1638,8 +1646,10 @@ void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, in
       fill_lift_row_kernel<<<(w + 255) / 256, 256, 0, c.stream>>>(d_local + (size_t)y * w, w, wcoarse.p + (size_t)((row0 + y) / k) * wc, k);
     }
     RDB_CK(cudaGetLastError());
+    st.topo4 = topo4;
     st.begin(d_local, w, hloc, wcoarse.p, wc, k, row0);
     lap0("band start (lifted)");
+    cst.topo4 = topo4;
     cst.begin(zc.p, wc, hc, wcoarse.p, wc, 1);
     cst.run();
     cst.track_dirty();
@@ -1648,6 +1658,7 @@ void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, in
   } else {
     if (gt) fill_f32(d_local, (size_t)w, inf);
     if (gb) fill_f32(d_local + (size_t)(hloc - 1) * w, (size_t)w, inf);
+    st.topo4 = topo4;
     st.begin(d_local, w, hloc);
   }
   int cycles = 0;

@@ -283,10 +283,14 @@ def coarse_fill(local_dem: "torch.Tensor", g_top: int, g_bot: int, row0: int, he
 
 def fill_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, solver_cls=None, group=None,
               max_rounds: int = 100000, return_stats: bool = False, band_rounds: Optional[int] = None,
-              multigrid: int = 0, row0: int = 0, height: int = 0, vcycle: int = 0):
+              multigrid: int = 0, row0: int = 0, height: int = 0, vcycle: int = 0, topology: str = "D8"):
     """Fill this rank's band.  ``local_dem`` is (g_top + owned + g_bot) x W with the ghost rows'
     contents ignored (they are initialised to +inf).  Returns (filled local raster incl. ghost rows,
     number of exchange rounds).  Collective: every rank of ``group`` must call it.
+
+    ``topology`` is that of ``FillDepressions``: ``"D8"`` or ``"D4"`` (PriorityFlood_Barnes2014<D4>, through
+    rdb200_mgpu_fill_depressions_d4_f32).  ``"D4"`` needs the C++ driver: the Python protocol (``solver_cls`` or
+    RDB_BAND_DRIVER=python) fills with D8 only and refuses it.
 
     ``multigrid`` = k >= 2 (with ``row0`` = global row of local row 0 and ``height`` = rows of the whole raster): start
     from the lifted fill of the k x k max-pooled raster (see :func:`coarse_fill`) instead of +inf -- an upper bound of
@@ -295,10 +299,16 @@ def fill_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, solver_cls=None
     lowered to the block maxima of the bands' surfaces (restriction; MAX all-reduce), relaxed again on every rank and
     handed back (prolongation: fine = min(fine, lifted)) -- a lake that is a little too high is lowered by a sweep
     across the COARSE raster instead of one tile row / halo exchange at a time."""
+    if topology not in ("D8", "D4"):
+        raise Exception("Unknown topology!")
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     import os
-    if solver_cls is None and os.environ.get("RDB_BAND_DRIVER", "cxx") != "python":
+    cxx = solver_cls is None and os.environ.get("RDB_BAND_DRIVER", "cxx") != "python"
+    if topology == "D4" and not cxx:
+        raise ValueError("fill_band(topology='D4') runs in the C++ band driver only; the Python band protocol "
+                         "(solver_cls, RDB_BAND_DRIVER=python) fills with D8")
+    if cxx:
         # the product path: the whole band protocol (multigrid start, halo exchanges, V-cycle corrections, termination)
         # runs in C++ over the library's communicator (csrc/fill.cu: mgpu_fill_band); in place on local_dem
         from . import _lib
@@ -316,8 +326,8 @@ def fill_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, solver_cls=None
                 height, row0 = h_, 0
         xr = C.c_int32(0)
         cm = lib_comm(group, local_dem.is_cuda)
-        _lib.check(_lib.lib().rdb200_mgpu_fill_depressions_d8_f32(cm.handle, local_dem.data_ptr(), w_, h_, int(g_top), int(g_bot),
-                                                                  int(row0), int(height), C.byref(xr)))
+        fn = _lib.lib().rdb200_mgpu_fill_depressions_d8_f32 if topology == "D8" else _lib.lib().rdb200_mgpu_fill_depressions_d4_f32
+        _lib.check(fn(cm.handle, local_dem.data_ptr(), w_, h_, int(g_top), int(g_bot), int(row0), int(height), C.byref(xr)))
         if return_stats:
             return local_dem, int(xr.value), _lib.stats()
         return local_dem, int(xr.value)
