@@ -255,6 +255,11 @@ RDB200_API int rdb200_dev_generate_fbm_f32(float *d_dem, int32_t width, int32_t 
  *   or, for the direction-grid pipeline after the fill (uint8 directions and int32 upslope-cell counts):
  *            rdb200_mgpu_d8_flow_directions_flats_f32(comm, d_band, d_dirs, W, rows, nodata, gt, gb, 0, NULL);
  *            rdb200_mgpu_d8_flow_accum_u8_i32(comm, d_dirs, d_area, W, rows, gt, gb, NULL);
+ *   or, for flow proportions, accumulation from them and terrain attributes of the band:
+ *            rdb200_mgpu_fm_method_f32(comm, 3, d_band, d_props, W, rows, nodata, gt, gb, 1.0);   (FM_Quinn)
+ *            rdb200_mgpu_flow_accumulation_props_f64(comm, d_props, d_accum, W, rows, gt, gb, NULL);
+ *            rdb200_mgpu_terrain_attribute_f32(comm, RDB200_TA_SLOPE_DEGREES, d_band, d_out, W, rows, nodata, -9999.f,
+ *                                              1.f, cell_x, cell_y, gt, gb);
  */
 typedef struct rdb200_comm rdb200_comm;
 enum { RDB200_MAX_F32 = 0, RDB200_MIN_F32 = 1, RDB200_MAX_I32 = 2, RDB200_SUM_I32 = 3 };
@@ -325,6 +330,33 @@ RDB200_API int rdb200_mgpu_d8_flow_directions_flats_f32(const rdb200_comm *comm,
 RDB200_API int rdb200_mgpu_d8_flow_accum_u8_i32(const rdb200_comm *comm, const uint8_t *d_band_dirs, int32_t *d_band_area,
                                                 int32_t width, int32_t local_rows, int32_t ghost_top, int32_t ghost_bottom,
                                                 int32_t *exchange_rounds);
+/* FM_D8 / FM_Tarboton / FM_D4 / FM_Holmgren (FM_Quinn = xparam 1.0) / FM_Freeman over row bands; method numbered as in
+ * rdb200_dev_fm_method_f32.  The call first exchanges the edge rows of d_band_dem, so on return its ghost rows hold the
+ * neighbours' edge rows; their contents on entry are ignored.  The owned rows of d_band_props9 (local_rows x width x 9)
+ * equal rdb200_dev_fm_method_f32 of the whole raster, bit for bit; its ghost rows are scratch.  Argument checks as
+ * rdb200_mgpu_resolve_flats_epsilon_f32, plus an unknown method, all before any communication. */
+RDB200_API int rdb200_mgpu_fm_method_f32(const rdb200_comm *comm, int32_t method, float *d_band_dem, float *d_band_props9,
+                                         int32_t width, int32_t local_rows, float nodata, int32_t ghost_top, int32_t ghost_bottom,
+                                         double xparam);
+/* TA_* (RDB200_TA_*) over row bands, with the arguments of rdb200_dev_terrain_attribute_f32.  The ghost rows of d_band_dem
+ * are refreshed as in rdb200_mgpu_fm_method_f32.  The owned rows of d_band_out equal rdb200_dev_terrain_attribute_f32 of
+ * the whole raster, bit for bit; its ghost rows are scratch.  An unknown attribute or a cell length that is not positive
+ * is an error before any communication. */
+RDB200_API int rdb200_mgpu_terrain_attribute_f32(const rdb200_comm *comm, int32_t attribute, float *d_band_dem, float *d_band_out,
+                                                 int32_t width, int32_t local_rows, float nodata_in, float nodata_out, float zscale,
+                                                 double cell_x, double cell_y, int32_t ghost_top, int32_t ghost_bottom);
+/* FlowAccumulation(props, accum) (include/richdem/methods/flow_accumulation_generic.hpp:33-100) over row bands, with the
+ * proportions supplied by the caller (local_rows x width x 9, as FM_* lay them out).  The ghost rows of d_band_props9 are
+ * not trusted: the call overwrites them with the neighbours' owned edge rows (one exchange of 36 B per cell and seam).
+ * d_band_accum_inout holds the weights on the owned rows on entry and the accumulation on return; its ghost rows are
+ * scratch.  As in rdb200_flow_accumulation_props_f64: NoData cells (slot 0 == -2) become -1, a share sent to a NoData cell
+ * is dropped, and flow out of raster-edge cells (global rows 0 and H-1, columns 0 and W-1) is ignored.  The owned rows equal
+ * the single-GPU call on the whole raster up to the order of the floating-point additions (bit for bit where every sum is
+ * exact, e.g. one-hot proportions with unit weights).  Argument checks as rdb200_mgpu_resolve_flats_epsilon_f32.
+ * *exchange_rounds (optional): walk rounds, each followed by one exchange of the flow that crossed a seam. */
+RDB200_API int rdb200_mgpu_flow_accumulation_props_f64(const rdb200_comm *comm, float *d_band_props9, double *d_band_accum_inout,
+                                                       int32_t width, int32_t local_rows, int32_t ghost_top, int32_t ghost_bottom,
+                                                       int32_t *exchange_rounds);
 
 /* ---- row-band (multi-GPU) fill: one band per GPU, halo rows exchanged by the caller -- */
 /* The band raster handed in is (band_rows + ghost rows) x width.  Its first and last rows are

@@ -273,6 +273,13 @@ _TERRAIN_ATTRIBS = {"slope_riserun": 0, "slope_percentage": 1, "slope_degrees": 
                     "curvature": 5, "planform_curvature": 6, "profile_curvature": 7}
 
 
+def _terrain_attrib_id(attrib: str) -> int:
+    """RDB200_TA_* number of a TerrainAttribute name (also used by sharded.terrain_attribute_band)."""
+    if attrib not in _TERRAIN_ATTRIBS:
+        raise Exception("Invalid TerrainAttributes attribute. Valid attributes are: " + ", ".join(_TERRAIN_ATTRIBS.keys()))
+    return _TERRAIN_ATTRIBS[attrib]
+
+
 def TerrainAttribute(dem: rdarray, attrib: str, zscale: float = 1.0) -> rdarray:
     """richdem.TerrainAttribute (wrappers/pyrichdem/richdem/__init__.py:735-794) over TA_* (methods/
     terrain_attributes.hpp:370-538): Horn (1981) slope / aspect, Zevenbergen & Thorne (1987) curvatures; float32
@@ -280,8 +287,7 @@ def TerrainAttribute(dem: rdarray, attrib: str, zscale: float = 1.0) -> rdarray:
     reference's wrap())."""
     if type(dem) is not rdarray:
         raise Exception("A richdem.rdarray or numpy.ndarray is required!")
-    if attrib not in _TERRAIN_ATTRIBS:
-        raise Exception("Invalid TerrainAttributes attribute. Valid attributes are: " + ", ".join(_TERRAIN_ATTRIBS.keys()))
+    attrib_id = _terrain_attrib_id(attrib)
     d = _dem_f32(dem, "TerrainAttribute")
     h, w = d.shape
     gt = dem.geotransform
@@ -290,7 +296,7 @@ def TerrainAttribute(dem: rdarray, attrib: str, zscale: float = 1.0) -> rdarray:
         gt = [0, 1, 0, 0, 0, -1]
     result = rdarray(np.zeros((h, w), np.float32), meta_obj=dem, no_data=-9999)
     _add_analysis(result, f"TerrainAttribute(dem, attrib={attrib}, zscale={zscale})")
-    _lib.check(_lib.lib().rdb200_terrain_attribute_f32(_TERRAIN_ATTRIBS[attrib], _lib.ptr(d), _lib.ptr(result), w, h,
+    _lib.check(_lib.lib().rdb200_terrain_attribute_f32(attrib_id, _lib.ptr(d), _lib.ptr(result), w, h,
                                                         _nodata_f32(dem), -9999.0, float(zscale), abs(float(gt[1])),
                                                         abs(float(gt[5]))))
     return result

@@ -88,6 +88,9 @@ SIGNATURES = {
     "rdb200_mgpu_resolve_flats_epsilon_f32": [_vp, _vp, _i32, _i32, _f32, _i32, _i32, C.POINTER(_i32)],
     "rdb200_mgpu_d8_flow_directions_flats_f32": [_vp, _vp, _vp, _i32, _i32, _f32, _i32, _i32, _i32, C.POINTER(_i32)],
     "rdb200_mgpu_d8_flow_accum_u8_i32": [_vp, _vp, _vp, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_mgpu_fm_method_f32": [_vp, _i32, _vp, _vp, _i32, _i32, _f32, _i32, _i32, C.c_double],
+    "rdb200_mgpu_terrain_attribute_f32": [_vp, _i32, _vp, _vp, _i32, _i32, _f32, _f32, _f32, C.c_double, C.c_double, _i32, _i32],
+    "rdb200_mgpu_flow_accumulation_props_f64": [_vp, _vp, _vp, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
     "rdb200_dev_fill_begin": [C.POINTER(_vp), _vp, _i32, _i32],
     "rdb200_dev_fill_begin_lifted": [C.POINTER(_vp), _vp, _i32, _i32, _vp, _i32, _i32, _i32],
     "rdb200_dev_maxpool_rows_f32": [_vp, _i32, _i32, _i32, _i32, _vp, _i32, _i32],

@@ -2219,6 +2219,7 @@ struct FaccState {
   DevBuf<uint8_t> code;
   DevBuf<float> rmax;
   DevBuf<float> props;
+  const float *pr = nullptr;  // the proportions the walk reads: props.p, or the caller's (begin_given_props)
   DevBuf<uint32_t> st;
   DevBuf<int> ghostcnt, fr0, fr1, cnt;
   bool prepared = false;
@@ -2296,8 +2297,33 @@ struct FaccState {
   // FM_* cell function tests NoData before the edge), so the walk drops flow into it as on one GPU.  Donor counts of
   // the owned rows are scattered here; the seam masks (set_ghost_codes) add the neighbours' shares to the edge rows.
   void begin_props(const float *d_dem, float nodata, double xparam, bool ones) {
-    Ctx &c = ctx();
     props.alloc(9 * n());
+    if (method == FA_BAND_D4) fm_d4_dev(d_dem, props.p, W, H, nodata);
+    else if (method == FA_BAND_HOLMGREN) fm_holmgren_dev(d_dem, props.p, W, H, nodata, xparam);
+    else fm_freeman_dev(d_dem, props.p, W, H, nodata, xparam);
+    init_props_walk(props.p, ones);
+  }
+
+  // FlowAccumulation(props, accum) of a band whose proportions the caller supplies (d_props, 9 floats per cell).  Only
+  // slot 0 of the ghost rows is read here, by the NoData test at the receiver, so the ghost rows must hold the neighbours'
+  // edge-row proportions (mgpu_flow_accumulation_props_band copies them in); deps_scatter_props_kernel skips the local
+  // edge rows, so the shares of those ghost cells are never counted, and the seam donor masks bring them in instead.
+  void begin_given_props(const float *d_props, double *d_accum, int w, int h, int ghost_top, int ghost_bottom) {
+    W = w;
+    H = h;
+    gt = ghost_top ? 1 : 0;
+    gb = ghost_bottom ? 1 : 0;
+    method = FA_BAND_D4;  // any proportions method: the walk and the seam protocol do not depend on it
+    mfd = true;
+    accum = d_accum;
+    if (h - gt - gb < 1) fail("facc_begin: band has no owned rows");
+    init_props_walk(d_props, false);
+  }
+
+  // donor counts of the proportions `p`, and the weights (ghost rows: empty parking slots; NoData: -1)
+  void init_props_walk(const float *p, bool ones) {
+    Ctx &c = ctx();
+    pr = p;
     st.alloc(n());
     ghostcnt.alloc(2 * (size_t)W);
     fr0.alloc(n());
@@ -2306,13 +2332,10 @@ struct FaccState {
     RDB_CK(cudaMemsetAsync(ghostcnt.p, 0, 2 * (size_t)W * sizeof(int), c.stream));
     RDB_CK(cudaMemsetAsync(cnt.p, 0, 4 * sizeof(int), c.stream));
     RDB_CK(cudaMemsetAsync(st.p, 0, n() * sizeof(uint32_t), c.stream));
-    if (method == FA_BAND_D4) fm_d4_dev(d_dem, props.p, W, H, nodata);
-    else if (method == FA_BAND_HOLMGREN) fm_holmgren_dev(d_dem, props.p, W, H, nodata, xparam);
-    else fm_freeman_dev(d_dem, props.p, W, H, nodata, xparam);
     const unsigned blocks = (unsigned)((n() + 255) / 256);
-    deps_scatter_props_kernel<<<blocks, 256, 0, c.stream>>>(props.p, st.p, W, H);
+    deps_scatter_props_kernel<<<blocks, 256, 0, c.stream>>>(pr, st.p, W, H);
     RDB_CK(cudaGetLastError());
-    band_init_props_accum_kernel<<<blocks, 256, 0, c.stream>>>(props.p, accum, W, H, gt, H - gb, ones ? 1 : 0);
+    band_init_props_accum_kernel<<<blocks, 256, 0, c.stream>>>(pr, accum, W, H, gt, H - gb, ones ? 1 : 0);
     RDB_CK(cudaGetLastError());
     count_launch(2);
   }
@@ -2364,8 +2387,14 @@ struct FaccState {
   void get_edge_codes(int which, uint8_t *d_code_row, float *d_rmax_row) {
     Ctx &c = ctx();
     if (mfd) {
-      band_seam_mask_kernel<<<(unsigned)((W + 255) / 256), 256, 0, c.stream>>>(props.p, d_code_row, W, edge_row(which),
-                                                                                which == 0 ? -1 : 1);
+      const int row = edge_row(which);
+      if (row == 0 || row == H - 1) {
+        // the band's one owned row is the raster's first or last row: raster-edge cells carry no flow (the walk skips
+        // them), so they announce none.  FM_* never give an edge cell flow; caller-supplied proportions may.
+        RDB_CK(cudaMemsetAsync(d_code_row, 0, W, c.stream));
+        return;
+      }
+      band_seam_mask_kernel<<<(unsigned)((W + 255) / 256), 256, 0, c.stream>>>(pr, d_code_row, W, row, which == 0 ? -1 : 1);
       RDB_CK(cudaGetLastError());
       count_launch();
       return;
@@ -2528,7 +2557,7 @@ struct FaccState {
     memset(&a, 0, sizeof(a));
     a.code = code.p;
     a.rmaxArr = rmax.p;
-    a.props = props.p;
+    a.props = pr;
     a.accum = accum;
     a.st = st.p;
     a.W = W;
@@ -2540,7 +2569,7 @@ struct FaccState {
     if (!prepared) {
       const unsigned blocks = (unsigned)((n() + 255) / 256);
       if (mfd)
-        band_mark_sources_props_kernel<<<blocks, 256, 0, c.stream>>>(props.p, st.p, W, H, gt, H - gb);
+        band_mark_sources_props_kernel<<<blocks, 256, 0, c.stream>>>(pr, st.p, W, H, gt, H - gb);
       else
         deps_gather_kernel<<<blocks, 256, 0, c.stream>>>(code.p, st.p, W, H, gt, H - gb, dinf ? 0 : 1);
       RDB_CK(cudaGetLastError());
@@ -2747,6 +2776,21 @@ void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, 
                   int method, double xparam, bool ones, int *xrounds) {
   FaccState A;
   A.begin(d_dem, d_accum, w, hloc, nodata, gt, gb, method, xparam, ones);
+  fa_band_rounds(comm, A, xrounds);
+}
+
+// FlowAccumulation(props, accum) over row bands, with the proportions supplied by the caller: the proportions protocol of
+// mgpu_fa_band (seam donor masks, the level walk, parcels parked in the ghost rows) on d_props instead of FM_x of a DEM.
+// The caller's ghost rows are not trusted: one exchange of the edge rows (36 B per cell) puts the neighbours' owned
+// proportions there first, so that the seam masks and the walk see which ghost cells are NoData.
+void mgpu_flow_accumulation_props_band(const rdb200_comm *comm, float *d_props, double *d_accum, int w, int hloc, int gt, int gb,
+                                       int *xrounds) {
+  const char *what = "mgpu_flow_accumulation_props";
+  if (!d_accum) fail("%s: null pointer", what);
+  check_band_args(what, comm, d_props, w, hloc, gt, gb);
+  exchange_band_rows(comm, d_props, 9 * sizeof(float), w, hloc, gt, gb);
+  FaccState A;
+  A.begin_given_props(d_props, d_accum, w, hloc, gt, gb);
   fa_band_rounds(comm, A, xrounds);
 }
 

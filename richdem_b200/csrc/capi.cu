@@ -638,6 +638,54 @@ int rdb200_mgpu_fa_method_f32_f64(const rdb200_comm *comm, const float *d_dem, d
   CAPI_END
 }
 
+// FM_x and TA_x over row bands: one exchange of the DEM's edge rows gives every owned cell its whole 3 x 3 neighbourhood,
+// and a local edge row is a raster edge row exactly when it is not a ghost row, so the single-GPU kernel on the local raster
+// gives the owned rows the single-GPU bits.  The arguments are checked before the exchange: a rank that fails must not
+// leave its neighbours waiting.
+int rdb200_mgpu_fm_method_f32(const rdb200_comm *comm, int32_t method, float *d_band_dem, float *d_band_props9, int32_t w,
+                              int32_t rows, float nodata, int32_t gt, int32_t gb, double xparam) {
+  CAPI_TRY
+  const char *what = "mgpu_fm_method";
+  if (!d_band_props9) fail("%s: null pointer", what);
+  check_band_args(what, comm, d_band_dem, w, rows, gt, gb);
+  check_dims(w, rows);
+  if (method < 0 || method > 4) fail("unknown flow metric %d", method);
+  CallScope cs((int64_t)w * rows);
+  exchange_band_rows(comm, d_band_dem, sizeof(float), w, rows, gt, gb);
+  fm_dispatch_dev(method, d_band_dem, d_band_props9, w, rows, nodata, xparam);
+  cs.done();
+  CAPI_END
+}
+
+int rdb200_mgpu_terrain_attribute_f32(const rdb200_comm *comm, int32_t attribute, float *d_band_dem, float *d_band_out, int32_t w,
+                                      int32_t rows, float nodata_in, float nodata_out, float zscale, double cell_x, double cell_y,
+                                      int32_t gt, int32_t gb) {
+  CAPI_TRY
+  const char *what = "mgpu_terrain_attribute";
+  if (!d_band_out) fail("%s: null pointer", what);
+  check_band_args(what, comm, d_band_dem, w, rows, gt, gb);
+  check_dims(w, rows);
+  if (attribute < RDB200_TA_SLOPE_RISERUN || attribute > RDB200_TA_PROFILE_CURVATURE) fail("unknown terrain attribute %d", attribute);
+  if (!(cell_x > 0) || !(cell_y > 0)) fail("terrain attribute: cell lengths must be positive (got %g x %g)", cell_x, cell_y);
+  CallScope cs((int64_t)w * rows);
+  exchange_band_rows(comm, d_band_dem, sizeof(float), w, rows, gt, gb);
+  terrain_attribute_dev(attribute, d_band_dem, d_band_out, w, rows, nodata_in, nodata_out, zscale, cell_x, cell_y);
+  cs.done();
+  CAPI_END
+}
+
+int rdb200_mgpu_flow_accumulation_props_f64(const rdb200_comm *comm, float *d_band_props9, double *d_band_accum_inout, int32_t w,
+                                            int32_t rows, int32_t gt, int32_t gb, int32_t *exchange_rounds) {
+  int xr = 0;
+  CAPI_TRY
+  check_dims(w, rows);
+  CallScope cs((int64_t)w * rows);
+  mgpu_flow_accumulation_props_band(comm, d_band_props9, d_band_accum_inout, w, rows, gt, gb, &xr);
+  cs.done();
+  if (exchange_rounds) *exchange_rounds = xr;
+  CAPI_END
+}
+
 int rdb200_mgpu_resolve_flats_epsilon_f32(const rdb200_comm *comm, float *d_band, int32_t w, int32_t rows, float nodata,
                                           int32_t gt, int32_t gb, int32_t *seam_iterations) {
   int it = 0;

@@ -168,6 +168,10 @@ void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, in
 // method: 0 D8, 1 Tarboton, 2 D4, 3 Holmgren (xparam; Quinn = 1.0), 4 Freeman (xparam)
 void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, int w, int hloc, float nodata, int gt, int gb,
                   int method, double xparam, bool ones, int *xrounds);
+// FlowAccumulation(props, accum) of caller-supplied 9-float proportions; the ghost rows of d_props are overwritten with the
+// neighbours' edge rows
+void mgpu_flow_accumulation_props_band(const rdb200_comm *comm, float *d_props, double *d_accum, int w, int hloc, int gt, int gb,
+                                       int *xrounds);
 void mgpu_resolve_flats_band(const rdb200_comm *comm, float *d_local, int w, int hloc, float nodata, int gt, int gb,
                              int *seam_iters);
 void mgpu_d8_flow_directions_flats_band(const rdb200_comm *comm, float *d_dem, uint8_t *d_dirs, int w, int hloc, float nodata,

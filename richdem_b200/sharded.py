@@ -399,11 +399,18 @@ def _fill_band_protocol(local_dem, g_top, g_bot, solver_cls, group, max_rounds, 
 def fa_method_id(method: Optional[str], exponent: Optional[float], dinf: bool = False) -> Tuple[int, float]:
     """(method number of the band entry points, exponent) for a FlowAccumulation method name.  ``method=None`` keeps
     the ``dinf`` switch: D-infinity if set, else D8.  Names and errors are those of :func:`richdem_b200.FlowAccumulation`."""
-    from . import _D4_METHODS, _D8_METHODS, _DINF_METHODS, _EXPONENT_METHODS, _OUT_OF_SCOPE_METHODS
+    from . import _DINF_METHODS
     if method is None:
         return (1 if dinf else 0), 0.0
     if dinf and method not in _DINF_METHODS:
         raise ValueError(f'dinf=True contradicts method "{method}"')
+    return _method_id(method, exponent, "FlowAccumulation")
+
+
+def _method_id(method: Optional[str], exponent: Optional[float], what: str) -> Tuple[int, float]:
+    """(method number, exponent) of a flow-metric name; the errors are those of :func:`richdem_b200.FlowAccumulation` or
+    :func:`richdem_b200.FlowProportions` (``what``), whose names are the same."""
+    from . import _D4_METHODS, _D8_METHODS, _DINF_METHODS, _EXPONENT_METHODS, _OUT_OF_SCOPE_METHODS
     if method in _D8_METHODS:
         return 0, 0.0
     if method in _DINF_METHODS:
@@ -414,12 +421,12 @@ def fa_method_id(method: Optional[str], exponent: Optional[float], dinf: bool = 
         return 3, 1.0
     if method in _EXPONENT_METHODS:
         if exponent is None:
-            raise Exception(f'FlowAccumulation method "{method}" requires an exponent!')
+            raise Exception(f'{what} method "{method}" requires an exponent!')
         return (3 if method == "Holmgren" else 4), float(exponent)
     if method in _OUT_OF_SCOPE_METHODS:
-        raise Exception(f'FlowAccumulation method "{method}" is outside the GPU hot path '
+        raise Exception(f'{what} method "{method}" is outside the GPU hot path '
                         "(random-walk metric; use the reference CPU implementation)")
-    raise Exception("Invalid FlowAccumulation method. Valid methods are: " +
+    raise Exception(f"Invalid {what} method. Valid methods are: " +
                     ", ".join(_DINF_METHODS + ("Quinn",) + _D8_METHODS + _D4_METHODS + _EXPONENT_METHODS +
                               _OUT_OF_SCOPE_METHODS))
 
@@ -790,3 +797,69 @@ def d8_flow_accum_band(local_dirs: "torch.Tensor", g_top: int, g_bot: int, group
     _lib.check(_lib.lib().rdb200_mgpu_d8_flow_accum_u8_i32(cm.handle, local_dirs.data_ptr(), area.data_ptr(), w, h, int(g_top),
                                                            int(g_bot), C.byref(xr)))
     return area, int(xr.value)
+
+
+# =================================================================================================
+# Flow proportions, accumulation from given proportions and terrain attributes over row bands
+# =================================================================================================
+def flow_proportions_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: float, method: Optional[str] = None,
+                          exponent: Optional[float] = None, group=None):
+    """FlowProportions over this rank's band.  ``local_dem`` is (g_top + owned + g_bot) x W; its ghost rows are refreshed
+    here with the neighbours' edge rows.  ``method`` / ``exponent`` and their errors are those of
+    :func:`richdem_b200.FlowProportions`.  Collective.  Returns float32 proportions of shape (local rows, W, 9) whose owned
+    rows are the single-GPU bits (ghost rows scratch)."""
+    from . import _lib
+    mid, xparam = _method_id(method, exponent, "FlowProportions")
+    assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
+    _lib.use_torch_stream()
+    h, w = local_dem.shape
+    props = torch.empty((h, w, 9), dtype=torch.float32, device=local_dem.device)
+    cm = lib_comm(group, local_dem.is_cuda)
+    _lib.check(_lib.lib().rdb200_mgpu_fm_method_f32(cm.handle, mid, local_dem.data_ptr(), props.data_ptr(), w, h, float(nodata),
+                                                    int(g_top), int(g_bot), xparam))
+    return props
+
+
+def flow_accum_from_props_band(local_props: "torch.Tensor", g_top: int, g_bot: int, weights: Optional["torch.Tensor"] = None,
+                               group=None):
+    """FlowAccumFromProps over this rank's band of float32 proportions, (g_top + owned + g_bot) x W x 9.  Their ghost rows
+    are not trusted: they are overwritten with the neighbours' edge rows.  ``weights`` (float64, (local rows, W)) defaults
+    to ones; when given it receives the accumulation in place.  NoData cells (slot 0 == -2) end as -1.  Collective.
+    Returns (float64 accumulation of the local shape, ghost rows scratch, exchange rounds)."""
+    from . import _lib
+    if local_props.dim() != 3 or local_props.shape[2] != 9:
+        raise RuntimeError("Array must have three dimensions with the last of size 9!")
+    assert _on_device(local_props) and local_props.dtype == torch.float32 and local_props.is_contiguous()
+    h, w = local_props.shape[0:2]
+    if weights is None:
+        acc = torch.ones((h, w), dtype=torch.float64, device=local_props.device)
+    else:
+        acc = weights
+        assert _on_device(acc) and acc.dtype == torch.float64 and acc.is_contiguous()
+        if tuple(acc.shape) != (h, w):
+            raise RuntimeError("Accumulation array must have same dimensions as proportions array!")
+    _lib.use_torch_stream()
+    xr = C.c_int32(0)
+    cm = lib_comm(group, local_props.is_cuda)
+    _lib.check(_lib.lib().rdb200_mgpu_flow_accumulation_props_f64(cm.handle, local_props.data_ptr(), acc.data_ptr(), w, h,
+                                                                  int(g_top), int(g_bot), C.byref(xr)))
+    return acc, int(xr.value)
+
+
+def terrain_attribute_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, attrib: str, nodata: float,
+                           zscale: float = 1.0, cell_x: float = 1.0, cell_y: float = 1.0, group=None):
+    """TerrainAttribute over this rank's band.  ``local_dem`` is (g_top + owned + g_bot) x W; its ghost rows are refreshed
+    here with the neighbours' edge rows.  ``attrib`` and its error are those of :func:`richdem_b200.TerrainAttribute`;
+    ``cell_x`` / ``cell_y`` are the cell lengths, |geotransform[1]| and |geotransform[5]|.  Collective.  Returns the
+    float32 attribute of the local shape, NoData -9999, whose owned rows are the single-GPU bits (ghost rows scratch)."""
+    from . import _lib, _terrain_attrib_id
+    aid = _terrain_attrib_id(attrib)
+    assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
+    _lib.use_torch_stream()
+    h, w = local_dem.shape
+    out = torch.empty((h, w), dtype=torch.float32, device=local_dem.device)
+    cm = lib_comm(group, local_dem.is_cuda)
+    _lib.check(_lib.lib().rdb200_mgpu_terrain_attribute_f32(cm.handle, aid, local_dem.data_ptr(), out.data_ptr(), w, h,
+                                                            float(nodata), -9999.0, float(zscale), float(cell_x), float(cell_y),
+                                                            int(g_top), int(g_bot)))
+    return out
