@@ -192,6 +192,83 @@ __device__ __forceinline__ void enqueue_tile(const FillArgs &a, RoundCtl *next, 
 
 __device__ __forceinline__ float min3f(float a, float b, float c) { return fminf(fminf(a, b), c); }
 
+// ---- staged first round: drain the lifted tile with column sweeps -----------------------------------------------------
+// A tile of the staged round starts from the lifted surface (constant pool x pool plateaus) and must drain nearly every
+// cell down towards Z, with all of its blocks dirty.  Before the dirty-block relaxation (which then runs unchanged from
+// SIDE_FULL and finishes the local fixed point), an N->S and an S->N sweep carry the drain down and up the whole tile:
+// one column per lane, a 64-row recurrence on the row before, W(x, y) <- min(W, max(Z, min of W(x-1..x+1, y -+ 1)))
+// (D4: W(x, y -+ 1) only -- a diagonal would lower cells below the D4 answer).  Every update is
+// W(c) <- min(W(c), max(Z(c), W(n))) for a neighbour n, which keeps W >= W* (W*(c) <= max(Z(c), W*(n))), leaves pinned
+// border cells (W = Z) and cells outside the raster (+inf) where they are, and only selects input values, so the result
+// is bit-identical.  Warps 0-1 run N->S over the top half while warps 2-3 run S->N over the bottom half, then they swap
+// halves carrying their last row in registers: both chains span the tile, and no cell has two writers in a phase (a
+// value read from a cell another warp owns may be old or new; both are upper bounds).
+// The tile's change flags and kmin are set for every cell the sweeps lower, as the block loop would have set them: a
+// tile edge lowered here and not touched again must still wake the neighbour that already read its lifted value in
+// this round.  (W->E / E->W row scans as warp scans of composed clamps were measured too: they cost more than they saved.)
+constexpr bool DRAIN_SWEEPS = TX == 64 && TY == 64 && FILL_THREADS == 128;
+
+template <bool TOPO4>
+__device__ __forceinline__ void fill_drain_sweeps(float *sW, const float *sZ, int y0, int H, int *sFlags, int *sKey) {
+  const unsigned FULL = 0xffffffffu;
+  const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
+  const int x = 32 * (wrp & 1) + lane;
+  const bool down = wrp < 2;
+  const int dy = down ? 1 : -1;
+  const bool ecol = x < 4 || x >= TX - 4;
+  unsigned long long rows = 0;                // tile rows where this thread lowered its column's cell
+  float kmin = __int_as_float(0x7f800000);   // lowest level it put on a cell of an edge block
+  int y = down ? 0 : TY - 1;
+  float p = sW[(y - dy + 1) * SP + PADL + x];  // the apron row
+#pragma unroll 1
+  for (int half = 0; half < 2; half++) {
+#pragma unroll 8
+    for (int s = 0; s < TY / 2; s++, y += dy) {
+      const float zz = sZ[y * TX + x];
+      float *cell = &sW[(y + 1) * SP + PADL + x];
+      const float w = *cell;
+      float m = p;
+      if (!TOPO4) {
+        float pl = __shfl_up_sync(FULL, p, 1), pr = __shfl_down_sync(FULL, p, 1);
+        const float *prow = &sW[(y - dy + 1) * SP + PADL + x];
+        if (lane == 0) pl = prow[-1];
+        if (lane == 31) pr = prow[1];
+        m = min3f(pl, p, pr);
+      }
+      const float nw = fminf(w, fmaxf(zz, m));
+      p = w;
+      if (nw < w) {
+        *cell = nw;
+        p = nw;
+        rows |= 1ull << y;
+        if (ecol || y < 4 || y >= TY - 4) kmin = fminf(kmin, nw);
+      }
+    }
+    __syncthreads();  // the other half's writers are done before it is swept
+  }
+  int f = 0;
+#pragma unroll
+  for (int by = 0; by < BYN; by++)
+    if ((rows >> (4 * by)) & 0xFull) f |= 1 << (12 + by);
+  if (rows & 1ull) f |= SIDE_N;
+  if (rows >> (TY - 1)) f |= SIDE_S;
+  if (x == 0 && rows) f |= SIDE_W | (rows & 1ull ? SIDE_NW : 0) | (rows >> (TY - 1) ? SIDE_SW : 0);
+  if (x == TX - 1 && rows) f |= SIDE_E | (rows & 1ull ? SIDE_NE : 0) | (rows >> (TY - 1) ? SIDE_SE : 0);
+  const int j1 = 1 - y0, j2 = (H - 2) - y0;  // raster rows 1 and H - 2
+  if (j1 >= 0 && j1 < TY && ((rows >> j1) & 1ull)) f |= 1 << 9;
+  if (j2 >= 0 && j2 < TY && ((rows >> j2) & 1ull)) f |= 1 << 10;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    f |= __shfl_xor_sync(FULL, f, o);
+    kmin = fminf(kmin, __shfl_xor_sync(FULL, kmin, o));
+  }
+  if (lane == 0 && f) {
+    atomicOr(sFlags, f);
+    if (f & 0xFF) atomicMin(sKey, f2ord(kmin));
+  }
+  // (the second half's __syncthreads above already published the swept window to the block loop)
+}
+
 // STEP = 0: depression filling,     new = min(W, max(Z, min8 W))
 // STEP = 1: geodesic distance,      new = min(W, max(Z, 1 + min8 W))   with Z = 0 on cells the flood
 //           may enter and +inf elsewhere (used for the flat-resolution gradients, csrc/flats.cu)
@@ -318,31 +395,55 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
       // with this round come from Wp.
       const float inf = __int_as_float(0x7f800000);
       const int nbdone = sNbDone;
-      for (int k = tid; k < SROWS * (SP / 4); k += FILL_THREADS) {
-        const int rr = k / (SP / 4), c4 = 4 * (k - rr * (SP / 4));
-        const int dy = rr == 0 ? -1 : (rr == SROWS - 1 ? 1 : 0), dx = c4 < PADL ? -1 : (c4 >= PADL + TX ? 1 : 0);
-        float4 v4;
-        if ((nbdone >> ((dy + 1) * 3 + dx + 1)) & 1) {
-          v4 = __ldcg(reinterpret_cast<const float4 *>(a.Wp + (size_t)(y0 + rr) * a.pitch + x0 + c4));
-        } else {
-          const int y = y0 + rr - 1, xb = x0 + c4 - PADL;  // raster coords of the first of the 4 cells
-          float v[4] = {inf, inf, inf, inf};
-          if (y >= 0 && y < a.H) {
-            const float *crow = a.coarse + (size_t)((y + a.yoff) / a.pool) * a.Wc;
-            const float *zrow = a.Z + (size_t)(y + a.zoy) * a.zpitch + a.zox;
-            const bool brow = y == 0 || y == a.H - 1;
-            // xb is a multiple of 4: with pool % 4 == 0 the 4 cells share one coarse block
-            const float c0 = (a.pool & 3) == 0 && xb >= 0 && xb < a.W ? __ldg(crow + xb / a.pool) : inf;
+      // each thread builds one group of 4 columns in every RSTEP-th row, so the coarse column is found once per tile
+      // and the coarse row advances by a fixed quotient and remainder: no division per group
+      constexpr int C4N = SP / 4, RSTEP = FILL_THREADS / C4N;
+      static_assert(RSTEP >= 1, "a CTA covers one row of the window");
+      if (tid < RSTEP * C4N) {
+        const int c4 = 4 * (tid % C4N);
+        int rr = tid / C4N;
+        const int dx = c4 < PADL ? -1 : (c4 >= PADL + TX ? 1 : 0);
+        const int xb = x0 + c4 - PADL;  // raster column of the first of the 4 cells (a multiple of 4)
+        const int cx = xb >= 0 ? xb / a.pool : 0, rx = xb - cx * a.pool;  // its coarse column and offset in it
+        const int yy = y0 + rr - 1 + a.yoff;  // >= -1
+        int cy = (yy + a.pool) / a.pool - 1, ry = yy - cy * a.pool;  // floor division
+        const int dq = RSTEP / a.pool, dr = RSTEP - dq * a.pool;
+        for (; rr < SROWS; rr += RSTEP) {
+          const int dy = rr == 0 ? -1 : (rr == SROWS - 1 ? 1 : 0);
+          float4 v4;
+          if ((nbdone >> ((dy + 1) * 3 + dx + 1)) & 1) {
+            v4 = __ldcg(reinterpret_cast<const float4 *>(a.Wp + (size_t)(y0 + rr) * a.pitch + x0 + c4));
+          } else {
+            const int y = y0 + rr - 1;
+            float v[4] = {inf, inf, inf, inf};
+            if (y >= 0 && y < a.H) {
+              const float *crow = a.coarse + (size_t)cy * a.Wc;
+              const float *zrow = a.Z + (size_t)(y + a.zoy) * a.zpitch + a.zox;
+              const bool brow = y == 0 || y == a.H - 1;
+              // with pool % 4 == 0 the 4 cells share one coarse block
+              const float c0 = (a.pool & 3) == 0 && xb >= 0 && xb < a.W ? __ldg(crow + cx) : inf;
+              int cc = cx, rc = rx;
 #pragma unroll
-            for (int j = 0; j < 4; j++) {
-              const int x = xb + j;
-              if (x >= 0 && x < a.W)
-                v[j] = brow || x == 0 || x == a.W - 1 ? __ldg(zrow + x) : (a.pool & 3) == 0 ? c0 : __ldg(crow + x / a.pool);
+              for (int j = 0; j < 4; j++) {
+                const int x = xb + j;
+                if (j > 0 && ++rc == a.pool) {
+                  rc = 0;
+                  cc++;
+                }
+                if (x >= 0 && x < a.W)
+                  v[j] = brow || x == 0 || x == a.W - 1 ? __ldg(zrow + x) : (a.pool & 3) == 0 ? c0 : __ldg(crow + cc);
+              }
             }
+            v4 = make_float4(v[0], v[1], v[2], v[3]);
           }
-          v4 = make_float4(v[0], v[1], v[2], v[3]);
+          *reinterpret_cast<float4 *>(&sW[rr * SP + c4]) = v4;
+          cy += dq;
+          ry += dr;
+          if (ry >= a.pool) {
+            ry -= a.pool;
+            cy++;
+          }
         }
-        *reinterpret_cast<float4 *>(&sW[rr * SP + c4]) = v4;
       }
     }
 #include "fill_relax_body.inc"
