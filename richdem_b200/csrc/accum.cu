@@ -1612,7 +1612,7 @@ __global__ void __launch_bounds__(256) band_apply_packed_kernel(unsigned long lo
 //      path from its receiver's slot leaves that tile.  The exit slots form a forest, solved by the packed countdown
 //      walk over slots; each exit's total outflow is added to the inflow of its receiver's slot.
 //   3. fa_tile_final_kernel: per tile, the codes again, every cell seeded with 1 plus the inflow on its slot, the
-//      in-tile accumulation, the result written as doubles.
+//      in-tile accumulation by pointer doubling (fa_tile_jump with SUM), the result written as doubles.
 // Per cell, HBM sees 4 B (DEM) + 2 x 1 B (codes) + 8 B (result); per slot (1/16 of the cells) 16 B of link data.  No
 // global atomic touches the cell raster.  All sums are integers < 2^31, so the result is exact whatever the order.
 // =================================================================================================
@@ -1647,66 +1647,69 @@ __device__ __forceinline__ bool fa_slot_cell(int s, int tw, int th, int &lx, int
   return k > 0 && k < th - 1 && (side == 2 || tw > 1);
 }
 
-// In-tile unit-weight accumulation in shared memory.  sCode: the tile's codes (row stride kFaT; kCodeNoData for NoData
-// and for cells beyond the raster), sWord: each data cell's seed, sQueue: room for the tile's sources and two counters
-// that are zero on entry.  Afterwards every data cell's word holds its seed plus the seeds of its upstream cells inside
-// the tile: the countdown protocol of the packed walk above, on shared memory.  The sources (cells without a donor in
-// the tile, listed before any walk can complete a cell) go into one queue per tile, and a thread whose walk has ended
-// takes the next one, so that a warp's time is about its share of the steps rather than the sum of its longest walks.
-__device__ __forceinline__ void fa_tile_accumulate(const uint8_t *sCode, unsigned long long *sWord, uint16_t *sQueue,
-                                                   int *sCount, int tw, int th) {
-  const int t = threadIdx.x;
-  for (int k = 0; k < kFaCells / 256; k++) {
-    const int c = t + 256 * k, lx = c & (kFaT - 1), ly = c / kFaT;
-    if (sCode[c] == kCodeNoData) continue;
-    unsigned deps = 0;
-#pragma unroll
-    for (int n = 1; n <= 8; n++) {
-      const int x = lx + d8dx(n), y = ly + d8dy(n);
-      if (x >= 0 && y >= 0 && x < tw && y < th && (sCode[y * kFaT + x] & 15) == d8_inverse(n)) deps++;
-    }
-    if (deps) sWord[c] += (unsigned long long)deps << 56;
-    else sQueue[atomicAdd(&sCount[0], 1)] = (uint16_t)c;
-  }
-  __syncthreads();
-  const int nsrc = sCount[0];
-  int cur = 0;
-  unsigned long long acc = 0;
-  bool walking = false;
-  for (;;) {  // one walk step per iteration, so that the lanes of a warp stay together
-    if (!walking) {
-      const int i = atomicAdd(&sCount[1], 1);
-      if (i >= nsrc) break;
-      cur = sQueue[i];
-      acc = sWord[cur];
-      walking = true;
-    }
-    const int d = sCode[cur] & 15;
-    const int x = (cur & (kFaT - 1)) + d8dx(d), y = cur / kFaT + d8dy(d);
-    if (d == 0 || x < 0 || y < 0 || x >= tw || y >= th) {  // no receiver, or it is in another tile
-      walking = false;
-      continue;
-    }
-    const int r = y * kFaT + x;
-    const unsigned long long old = atomicAdd(&sWord[r], acc - kPkOne);
-    if ((old >> 56) != 1ull) {  // other donors are still to come: the last one carries on
-      walking = false;
-      continue;
-    }
-    acc = (old & kPkVal) + acc;
-    cur = r;
-  }
-  __syncthreads();
+// Flags of a root in a tile's parent array (cell indices need 12 bits): the path leaves the tile here, or it ends here
+// (no receiver, or NoData).  An entry that carries a flag names the root of its cell's path.
+constexpr int kFaRootExit = 0x8000, kFaRootEnd = 0x4000, kFaRoot = kFaRootExit | kFaRootEnd;
+
+// the parent array entry of tile cell c with code cd: its in-tile receiver, or c itself flagged as a root
+__device__ __forceinline__ int fa_tile_parent(int c, int cd, int tw, int th) {
+  const int d = cd & 15;
+  if (cd == kCodeNoData || d == 0) return c | kFaRootEnd;
+  const int x = (c & (kFaT - 1)) + d8dx(d), y = c / kFaT + d8dy(d);
+  if (x < 0 || y < 0 || x >= tw || y >= th) return c | kFaRootExit;
+  return y * kFaT + x;
 }
 
-// Flags of a root in fa_tile_codes_kernel's parent array (cell indices need 12 bits): the path leaves the tile here, or it
-// ends here (no receiver, or NoData).
-constexpr int kFaRootExit = 0x8000, kFaRootEnd = 0x4000;
+// Pointer jumping over a tile's parent array sPar, 16 cells per thread: bit k of `live` says that cell t + 256 k's
+// entry carries no flag.  After r rounds such an *exact* entry names p_r, the cell exactly 2^r steps down its in-tile
+// path; a round sets p[c] = p[p[c]], and an entry that reads a flag has reached its root in fewer steps and keeps it
+// from then on.  The loop ends when every entry names its flagged root, after at most ceil(log2 4096) = 12 rounds.
+// With SUM, sAcc holds every cell's weight on entry and its in-tile accumulation on exit.  Writing A_r(c) for the sum of
+// the weights of the cells fewer than 2^r steps upstream of c (c included),
+//     A_{r+1}(c) = A_r(c) + sum of A_r(d) over the cells d with an exact p_r(d) = c,
+// since every cell 2^r to 2^{r+1} - 1 steps upstream of c is fewer than 2^r steps upstream of exactly one such d.  Each
+// round reads A_r and p_r before anything is added or replaced, so it takes two barriers; a cell's work is one shared
+// atomicAdd per round in which its entry is exact, about log2 of its distance to the root, instead of a walk as long as
+// the path.  Without SUM any ancestor read is as good as the one a round intended, so the entry is replaced in place,
+// one barrier per round.
+template <bool SUM>
+__device__ __forceinline__ void fa_tile_jump(uint16_t *sPar, unsigned *sAcc, unsigned live) {
+  constexpr int kPer = kFaCells / 256;
+  const int t = threadIdx.x;
+  while (__syncthreads_or(live)) {
+    unsigned pq[kPer], a[kPer];  // SUM: [p_r(c) | p_r(p_r(c)) << 16] and A_r(c), kept across the barrier
+#pragma unroll
+    for (int k = 0; k < kPer; k++) {
+      if (live >> k & 1) {
+        const int c = t + 256 * k, p = sPar[c], q = sPar[p];
+        if (SUM) {
+          pq[k] = (unsigned)p | (unsigned)q << 16;
+          a[k] = sAcc[c];
+        } else {
+          sPar[c] = (uint16_t)q;
+          if (q & kFaRoot) live &= ~(1u << k);
+        }
+      }
+    }
+    if (SUM) {
+      __syncthreads();
+#pragma unroll
+      for (int k = 0; k < kPer; k++) {
+        if (live >> k & 1) {
+          const int q = pq[k] >> 16;
+          atomicAdd(&sAcc[pq[k] & 0xffffu], a[k]);
+          sPar[t + 256 * k] = (uint16_t)q;
+          if (q & kFaRoot) live &= ~(1u << k);
+        }
+      }
+    }
+  }
+}
 
 // Pass 1 needs no accumulation.  Per slot the link solve needs the exit slot where its in-tile path leaves the tile, and
 // per exit slot the number of the tile's data cells whose in-tile path ends there.  Both follow from each cell's *root*,
-// the last in-tile cell on its path, which pointer jumping finds in at most ceil(log2 4096) = 12 rounds of shared-memory
-// loads; a walk would take as many dependent steps as the tile's longest in-tile path.
+// the last in-tile cell on its path, which pointer jumping (fa_tile_jump without SUM) finds in at most 12 rounds of
+// shared-memory loads; a walk would take as many dependent steps as the tile's longest in-tile path.
 __global__ void __launch_bounds__(256) fa_tile_codes_kernel(const float *__restrict__ dem, uint8_t *__restrict__ code,
                                                              int *__restrict__ link, unsigned long long *__restrict__ lword,
                                                              unsigned *__restrict__ inflow, int W, int H, float nodata,
@@ -1721,85 +1724,77 @@ __global__ void __launch_bounds__(256) fa_tile_codes_kernel(const float *__restr
   const int bx = tile % tiles_x, by = tile / tiles_x;
   const int x0 = bx * kFaT, y0 = by * kFaT;
   const int tw = fa_side(W - x0), th = fa_side(H - y0);
+  // NoData (and the apron beyond the raster) is held as the NaN kFaNoDataBits, every NaN of the DEM as the canonical
+  // one: as a neighbour any NaN fails every comparison of the steepest-descent scan, which is exactly "skip NoData", and
+  // the cell's own NoData test is one integer compare.  A NaN no-data value matches nothing, as in the reference.
+  constexpr unsigned kFaNoDataBits = 0x7fffffffu;
   for (int i = t; i < kWin * kWin; i += 256) {
     const int wy = i / kWin, wx = i - wy * kWin;
     const int gy = y0 - 1 + wy, gx = x0 - 1 + wx;
-    sDem[i] = (gy >= 0 && gy < H && gx >= 0 && gx < W) ? __ldg(dem + (size_t)gy * W + gx) : nodata;
+    float v = __uint_as_float(kFaNoDataBits);
+    if (gy >= 0 && gy < H && gx >= 0 && gx < W) {
+      v = __ldg(dem + (size_t)gy * W + gx);
+      v = v == nodata ? __uint_as_float(kFaNoDataBits) : v != v ? __uint_as_float(0x7fc00000u) : v;
+    }
+    sDem[i] = v;
   }
   __syncthreads();
   // flow codes, the rule of fa_d8_prep_rolling_kernel: the first strictly lowest data neighbour; raster-border cells have
-  // no receiver.  Thread t: column t % 64, a strip of 16 rows, a rolling 3 x 3 register window.
+  // no receiver.  Thread t: columns 4 (t % 16) .. + 3, a strip of 4 rows, a rolling 3 x 6 register window; the 4 codes of
+  // a row leave as one 32-bit word.
   {
-    const int lx = t & (kFaT - 1), ly0 = (t / kFaT) * (kFaT / 4);
-    float a[3][3];
+    const int lx0 = (t & 15) * 4, ly0 = (t >> 4) * 4;
+    float a[3][6];
 #pragma unroll
     for (int j = 1; j < 3; j++)
 #pragma unroll
-      for (int k = 0; k < 3; k++) a[j][k] = sDem[(ly0 + j - 1) * kWin + lx + k];
-    for (int j = 0; j < kFaT / 4; j++) {
-      const int ly = ly0 + j;
+      for (int k = 0; k < 6; k++) a[j][k] = sDem[(ly0 + j - 1) * kWin + lx0 + k];
 #pragma unroll
-      for (int k = 0; k < 3; k++) {
+    for (int j = 0; j < 4; j++) {
+      const int ly = ly0 + j, gy = y0 + ly;
+#pragma unroll
+      for (int k = 0; k < 6; k++) {
         a[0][k] = a[1][k];
         a[1][k] = a[2][k];
-        a[2][k] = sDem[(ly + 2) * kWin + lx + k];
+        a[2][k] = sDem[(ly + 2) * kWin + lx0 + k];
       }
-      const float e = a[1][1];
-      const int gx = x0 + lx, gy = y0 + ly;
-      int cd = 0;
-      if (lx >= tw || ly >= th || e == nodata) {
-        cd = kCodeNoData;
-      } else if (!(gx == 0 || gy == 0 || gx == W - 1 || gy == H - 1)) {
-        // neighbours n = 1..8 : W, NW, N, NE, E, SE, S, SW.  Starting the running minimum at the cell's own value folds
-        // the reference's `>= e` skip into it (capped at FLT_MAX, the reference's starting value)
-        const float ne[9] = {0.f, a[1][0], a[0][0], a[0][1], a[0][2], a[1][2], a[2][2], a[2][1], a[2][0]};
-        float lowest = fminf(e, 3.402823466e+38f);
+      unsigned word = 0;
 #pragma unroll
-        for (int n = 1; n <= 8; n++) {
-          const float v = ne[n];
-          if (v < lowest && v != nodata) {
-            lowest = v;
-            cd = n;
+      for (int k = 0; k < 4; k++) {
+        const int lx = lx0 + k, gx = x0 + lx;
+        const float e = a[1][k + 1];
+        int cd = 0;
+        if (lx >= tw || ly >= th || __float_as_uint(e) == kFaNoDataBits) {
+          cd = kCodeNoData;
+        } else if (!(gx == 0 || gy == 0 || gx == W - 1 || gy == H - 1)) {
+          // neighbours n = 1..8 : W, NW, N, NE, E, SE, S, SW.  Starting the running minimum at the cell's own value
+          // folds the reference's `>= e` skip into it (capped at FLT_MAX, the reference's starting value)
+          const float ne[9] = {0.f, a[1][k], a[0][k], a[0][k + 1], a[0][k + 2], a[1][k + 2], a[2][k + 2], a[2][k + 1], a[2][k]};
+          float lowest = fminf(e, 3.402823466e+38f);
+#pragma unroll
+          for (int n = 1; n <= 8; n++) {
+            if (ne[n] < lowest) {
+              lowest = ne[n];
+              cd = n;
+            }
           }
         }
+        word |= (unsigned)cd << (8 * k);
       }
-      sCode[ly * kFaT + lx] = (uint8_t)cd;
+      *reinterpret_cast<unsigned *>(&sCode[ly * kFaT + lx0]) = word;
     }
   }
   __syncthreads();  // the DEM window is dead from here on
   reinterpret_cast<uint4 *>(code + (size_t)tile * kFaCells)[t] = reinterpret_cast<const uint4 *>(sCode)[t];
-  // parents: a cell's in-tile receiver; a root holds its own index and its flag.  Bit k of `live`: cell t + 256 k has no
-  // root yet.
   uint16_t *sPar = reinterpret_cast<uint16_t *>(sDem);
   unsigned live = 0;
 #pragma unroll
   for (int k = 0; k < kFaCells / 256; k++) {
-    const int c = t + 256 * k, cd = sCode[c], d = cd & 15;
-    int p = c | kFaRootEnd;
-    if (cd != kCodeNoData && d != 0) {
-      const int x = (c & (kFaT - 1)) + d8dx(d), y = c / kFaT + d8dy(d);
-      if (x < 0 || y < 0 || x >= tw || y >= th) {
-        p = c | kFaRootExit;
-      } else {
-        p = y * kFaT + x;
-        live |= 1u << k;
-      }
-    }
+    const int c = t + 256 * k, p = fa_tile_parent(c, sCode[c], tw, th);
     sPar[c] = (uint16_t)p;
+    if (!(p & kFaRoot)) live |= 1u << k;
   }
-  // Pointer jumping, p[c] = p[p[c]], until every cell holds its flagged root.  Only the owner writes a cell's entry, and
-  // every value anyone reads is an ancestor on the path (a newer one is further up), so the barrier per round is all the
-  // ordering needed; it bounds the rounds by the log of the longest in-tile path.  Paths descend, so there are no cycles.
-  while (__syncthreads_or(live)) {
-#pragma unroll
-    for (int k = 0; k < kFaCells / 256; k++) {
-      if (live >> k & 1) {
-        const int c = t + 256 * k, q = sPar[sPar[c]];
-        sPar[c] = (uint16_t)q;
-        if (q & (kFaRootExit | kFaRootEnd)) live &= ~(1u << k);
-      }
-    }
-  }
+  fa_tile_jump<false>(sPar, nullptr, live);
 #pragma unroll
   for (int k = 0; k < kFaCells / 256; k++) {
     const int r = sPar[t + 256 * k];
@@ -1871,26 +1866,43 @@ __global__ void __launch_bounds__(256) fa_link_walk_kernel(const int *__restrict
 __global__ void __launch_bounds__(256) fa_tile_final_kernel(const uint8_t *__restrict__ code,
                                                              const unsigned *__restrict__ inflow, double *__restrict__ accum,
                                                              int W, int H, int tiles_x) {
-  __shared__ __align__(16) unsigned long long sWord[kFaCells];
+  constexpr unsigned kNoDataAcc = 0xffffffffu;  // a NoData cell's sum: no data cell's sum comes near it (< 2^31)
+  __shared__ __align__(16) unsigned sAcc[kFaCells];
+  __shared__ __align__(16) uint16_t sPar[kFaCells];
   __shared__ __align__(16) uint8_t sCode[kFaCells];
-  __shared__ uint16_t sQueue[kFaCells];
-  __shared__ int sCount[2];
   const int t = threadIdx.x, tile = blockIdx.x;
   const int bx = tile % tiles_x, by = tile / tiles_x;
   const int x0 = bx * kFaT, y0 = by * kFaT;
   const int tw = fa_side(W - x0), th = fa_side(H - y0);
-  if (t < 2) sCount[t] = 0;
   reinterpret_cast<uint4 *>(sCode)[t] = __ldg(reinterpret_cast<const uint4 *>(code + (size_t)tile * kFaCells) + t);
-  for (int c = t; c < kFaCells; c += 256) sWord[c] = 1;
+  __syncthreads();
+  // weights: 1 per data cell (plus the inflow on its slot, below), none for NoData, whose entry is a root from the start
+  unsigned live = 0;
+#pragma unroll
+  for (int k = 0; k < kFaCells / 256; k++) {
+    const int c = t + 256 * k, cd = sCode[c], p = fa_tile_parent(c, cd, tw, th);
+    sPar[c] = (uint16_t)p;
+    sAcc[c] = cd == kCodeNoData ? kNoDataAcc : 1u;
+    if (!(p & kFaRoot)) live |= 1u << k;
+  }
   __syncthreads();
   int lx, ly;
-  if (fa_slot_cell(t, tw, th, lx, ly)) sWord[ly * kFaT + lx] += __ldg(inflow + (size_t)tile * kFaSlots + t);
-  __syncthreads();
-  fa_tile_accumulate(sCode, sWord, sQueue, sCount, tw, th);
-  for (int c = t; c < kFaCells; c += 256) {
+  if (fa_slot_cell(t, tw, th, lx, ly) && sCode[ly * kFaT + lx] != kCodeNoData)
+    sAcc[ly * kFaT + lx] += __ldg(inflow + (size_t)tile * kFaSlots + t);
+  fa_tile_jump<true>(sPar, sAcc, live);
+  // two cells per thread and step, one 16-byte store where the row's address allows it (odd widths, unaligned rasters)
+  for (int c = 2 * t; c < kFaCells; c += 512) {
     const int cx = c & (kFaT - 1), cy = c / kFaT;
-    if (cx < tw && cy < th)
-      accum[(size_t)(y0 + cy) * W + x0 + cx] = sCode[c] == kCodeNoData ? -1.0 : (double)(sWord[c] & kPkVal);  // -1: flow_accumulation_generic.hpp:95-97
+    if (cx >= tw || cy >= th) continue;
+    const unsigned s0 = sAcc[c], s1 = sAcc[c + 1];
+    const double a0 = s0 == kNoDataAcc ? -1.0 : (double)s0, a1 = s1 == kNoDataAcc ? -1.0 : (double)s1;  // -1: flow_accumulation_generic.hpp:95-97
+    double *out = accum + (size_t)(y0 + cy) * W + x0 + cx;
+    if (cx + 1 < tw && ((uintptr_t)out & 15) == 0) {
+      *reinterpret_cast<double2 *>(out) = make_double2(a0, a1);
+    } else {
+      out[0] = a0;
+      if (cx + 1 < tw) out[1] = a1;
+    }
   }
 }
 
