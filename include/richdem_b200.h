@@ -205,6 +205,10 @@ RDB200_API int rdb200_fa_tarboton_f32_f64(const float *dem, double *accum_inout,
 
 /* ---- device entry points (pointers into HBM of the current device) ----------------- */
 
+/* Depression filling in place.  While the call runs, d_dem holds intermediate water levels (when width is a multiple
+ * of 4 and d_dem is 16-byte aligned, the fill relaxes its water surface in the raster itself and keeps the elevations
+ * in a scratch copy), so nothing else may read or write it meanwhile.  If the call returns an error, the contents of
+ * d_dem are unspecified. */
 RDB200_API int rdb200_dev_fill_depressions_d8_f32(float *d_dem, int32_t width, int32_t height);
 RDB200_API int rdb200_dev_fill_depressions_d4_f32(float *d_dem, int32_t width, int32_t height);
 RDB200_API int rdb200_dev_resolve_flats_epsilon_f32(float *d_dem, int32_t width, int32_t height, float nodata);

@@ -57,7 +57,7 @@ struct Params {
   int64_t fill_max_iters = 0;   // 0 = relax every tile visit to its local fixed point
   int64_t fill_rounds_per_sync = 16;
   int64_t fill_use_tma = 1;     // 0: plain ld.global staging (debug aid)
-  int64_t fill_external_z = 1;  // single-GPU fill: Z from the caller's raster, round 1 staged from the lifted start (0: padded Z copy)
+  int64_t fill_external_z = 1;  // single-GPU fill: W relaxed in the caller's raster, round 1 staged from the lifted start (0: padded W and Z)
   int64_t fill_ordered = 1;       // admit tiles by rising water level (device-side feedback on the level)
   int64_t fill_order_rounds = 0;  // rounds the level schedule spans (0: 0.8 x tiles across the raster)
   int64_t fill_band_rounds = 0;   // row-band mode: rounds per rdb200_dev_fill_run call (0: to convergence)

@@ -83,17 +83,22 @@ struct FillDev {
 };
 
 struct FillArgs {
-  // Z of cell (x, y) is Z[(y + zoy) * zpitch + x + zox]: the padded copy (pitch, 1, PADL), or the caller's w x h raster
-  // itself (zext: row stride W, no offsets; cells outside the raster read as +inf)
+  // Z of cell (x, y) is Z[(y + zoy) * zpitch + x + zox] and its water level Wp[(y + woy) * pitch + x + wox].  Padded
+  // layout: both padded arrays (pitch, offsets PADL and 1).  In place (`inplace`): W is the caller's w x h raster and Z a
+  // compact w x h array (row stride W, no offsets); cells outside the raster read as +inf.
   const float *Z;
-  int zpitch, zox, zoy, zext;
-  // round 1 of a lifted start: W is built from the coarse surface instead of loaded (null: load it); `staged` flags the
-  // tiles whose cells are in Wp already
+  int zpitch, zox, zoy;
+  int inplace;
+  // round 1 of a lifted start (in place only): W is built from the coarse surface instead of loaded (null: load it);
+  // `staged` flags the tiles whose cells are in W already.  Z is then still the caller's raster, and every tile saves its
+  // Z to `zcopy` (the compact Z of the later rounds) before its W overwrites it.
   const float *coarse;
   int Wc, pool, yoff;
   int *staged;
+  float *zcopy;
   float *Wp;
   int pitch;  // floats
+  int wox, woy;
   int W, H;
   int tilesX, tilesY;
   int *list0, *list1;
@@ -149,6 +154,17 @@ __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *m
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
+// shared -> global tile store (cells of the box outside the tensor are not written), committed as its own bulk group
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, int c0, int c1, const void *smem_src) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];" ::"l"((unsigned long long)map),
+               "r"(c0), "r"(c1), "r"(smem_u32(smem_src))
+               : "memory");
+  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
+// the shared memory of every bulk store issued by this thread may be overwritten
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// every bulk store issued by this thread is complete
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ---- the sweep kernel --------------------------------------------------------------------
 // A tile is 16x16 "blocks" of 4x4 cells.  Relaxation is driven by a compacted list of dirty
@@ -273,12 +289,13 @@ __device__ __forceinline__ void fill_drain_sweeps(float *sW, const float *sZ, in
 // STEP = 1: geodesic distance,      new = min(W, max(Z, 1 + min8 W))   with Z = 0 on cells the flood
 //           may enter and +inf elsewhere (used for the flat-resolution gradients, csrc/flats.cu)
 // TOPO4: the 4-neighbour (D4) stencil of FillDepressions<Topology::D4>; corner aprons are then never read
-// STAGE: round 1 of a staged lifted start (a.coarse): W is built from the coarse surface, not loaded, and every row is
-//        written back (a template parameter so that the later rounds keep their registers)
+// STAGE: round 1 of a staged lifted start (a.coarse): W is built from the coarse surface, not loaded, every row is
+//        written back, and the tile's Z is saved to a.zcopy through mapZout (a template parameter so that the later
+//        rounds keep their registers)
 template <int STEP, bool TOPO4 = false, bool STAGE = false>
 __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
     fill_sweep_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__ CUtensorMap mapZ,
-                      const FillArgs a) {
+                      const __grid_constant__ CUtensorMap mapZout, const FillArgs a) {
   __shared__ __align__(128) float sW[SROWS * SP];
   __shared__ __align__(128) float sZ[TY * TX];
   __shared__ __align__(8) unsigned long long mbar;
@@ -291,7 +308,7 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
   __shared__ int sFlags;
   __shared__ int sKey;
   __shared__ int sProf[2];
-  __shared__ int sNbDone;  // staged round: neighbours (bit (dy + 1) * 3 + dx + 1) whose cells are in Wp already
+  __shared__ int sNbDone;  // staged round: neighbours (bit (dy + 1) * 3 + dx + 1) whose cells are in W already
 
   const int tid = threadIdx.x;
   const int r = a.round;
@@ -353,31 +370,36 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
                 *reinterpret_cast<volatile int *>(&a.staged[ty * a.tilesX + tx]))
               nb |= 1 << ((dy + 1) * 3 + dx + 1);
           }
-        __threadfence();  // their Wp stores are read after their flags
+        __threadfence();  // their W stores are read after their flags
         sNbDone = nb;
       }
     }
     if (a.use_tma) {
       if (tid == 0) {
         fence_proxy_async();  // order earlier generic-proxy smem accesses before the async writes
+        if (STAGE) bulk_wait_read();  // the previous tile's Z store has read sZ
         mbar_arrive_expect_tx(&mbar, (stage ? 0u : W_TILE_BYTES) + Z_TILE_BYTES);
-        if (!stage) tma_load_2d(sW, &mapW, x0, y0, &mbar);  // padded cols x0..x0+71, rows y0..y0+65
+        // the window: cells x0-4..x0+67, y0-1..y0+64 (in place, those outside the raster arrive as zeros: see below)
+        if (!stage) tma_load_2d(sW, &mapW, x0 - PADL + a.wox, y0 - 1 + a.woy, &mbar);
         tma_load_2d(sZ, &mapZ, x0 + a.zox, y0 + a.zoy, &mbar);  // the 64x64 interior
       }
     } else {
+      // (W % 4 == 0 in place: a float4 lies wholly inside or wholly outside the raster)
+      const float inf = __int_as_float(0x7f800000);
       if (!stage) {
         for (int k = tid; k < SROWS * (SP / 4); k += FILL_THREADS) {
           const int rr = k / (SP / 4), cc = k - rr * (SP / 4);
+          const int y = y0 + rr - 1, x = x0 + 4 * cc - PADL;  // raster cell of the group's first float
           reinterpret_cast<float4 *>(sW)[k] =
-              __ldcg(reinterpret_cast<const float4 *>(a.Wp + (size_t)(y0 + rr) * a.pitch + x0) + cc);
+              a.inplace && (y < 0 || y >= a.H || x < 0 || x >= a.W)
+                  ? make_float4(inf, inf, inf, inf)
+                  : __ldcg(reinterpret_cast<const float4 *>(a.Wp + (size_t)(y + a.woy) * a.pitch + x + a.wox));
         }
       }
-      const float inf = __int_as_float(0x7f800000);
       for (int k = tid; k < TY * (TX / 4); k += FILL_THREADS) {
         const int rr = k / (TX / 4), cc = k - rr * (TX / 4);
-        // (W % 4 == 0 in zext mode: a float4 lies wholly inside or wholly outside the raster)
         reinterpret_cast<float4 *>(sZ)[k] =
-            a.zext && (y0 + rr >= a.H || x0 + 4 * cc >= a.W)
+            a.inplace && (y0 + rr >= a.H || x0 + 4 * cc >= a.W)
                 ? make_float4(inf, inf, inf, inf)
                 : __ldg(reinterpret_cast<const float4 *>(a.Z + (size_t)(y0 + a.zoy + rr) * a.zpitch + x0 + a.zox) + cc);
       }
@@ -392,7 +414,9 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
     if (stage) {
       // The start W0 of fill_init_kernel<true>, built here instead of loaded: Z on the raster border, +inf outside the
       // raster, elsewhere the coarse level of the cell's pool x pool block.  Apron cells of a neighbour that is done
-      // with this round come from Wp.
+      // with this round come from W (the caller's raster, where that neighbour has stored its cells).  The raster's
+      // border cells are read from Z, i.e. the same raster, which a neighbour may be writing right now: coherent loads,
+      // and a border cell holds the same bits either way (W = Z there).
       const float inf = __int_as_float(0x7f800000);
       const int nbdone = sNbDone;
       // each thread builds one group of 4 columns in every RSTEP-th row, so the coarse column is found once per tile
@@ -411,8 +435,11 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
         for (; rr < SROWS; rr += RSTEP) {
           const int dy = rr == 0 ? -1 : (rr == SROWS - 1 ? 1 : 0);
           float4 v4;
-          if ((nbdone >> ((dy + 1) * 3 + dx + 1)) & 1) {
-            v4 = __ldcg(reinterpret_cast<const float4 *>(a.Wp + (size_t)(y0 + rr) * a.pitch + x0 + c4));
+          // Only the neighbour's cells inside the raster are read: beside the last tile row its rows, and above or below
+          // a partial last tile column its columns, may lie outside (the groups of 4 lie wholly on one side: W % 4 == 0).
+          // Those take the branch below, which makes them +inf as the padded layout's padding would be.
+          if (((nbdone >> ((dy + 1) * 3 + dx + 1)) & 1) && y0 + rr - 1 < a.H && xb < a.W) {
+            v4 = __ldcg(reinterpret_cast<const float4 *>(a.Wp + (size_t)(y0 + rr - 1 + a.woy) * a.pitch + xb + a.wox));
           } else {
             const int y = y0 + rr - 1;
             float v[4] = {inf, inf, inf, inf};
@@ -431,7 +458,7 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
                   cc++;
                 }
                 if (x >= 0 && x < a.W)
-                  v[j] = brow || x == 0 || x == a.W - 1 ? __ldg(zrow + x) : (a.pool & 3) == 0 ? c0 : __ldg(crow + cc);
+                  v[j] = brow || x == 0 || x == a.W - 1 ? __ldcg(zrow + x) : (a.pool & 3) == 0 ? c0 : __ldg(crow + cc);
               }
             }
             v4 = make_float4(v[0], v[1], v[2], v[3]);
@@ -456,15 +483,21 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
     __syncthreads();
     const int fl = sFlags;
     const int rowch = (fl >> 12) & 0xFFFF;
-    // a staged round writes every row: it is what initialises the tile's cells in Wp
+    // a staged round writes every row: it is what initialises the tile's cells in W
     const int rowout = stage ? (1 << BYN) - 1 : rowch;
     if (rowout) {
-      // coalesced float4 write-back of the block rows (4 cell rows x 64) that hold a change
+      // coalesced float4 write-back of the block rows (4 cell rows x 64) that hold a change; in place, of their cells
+      // inside the raster
       for (int k = tid; k < TY * (TX / 4); k += FILL_THREADS) {
         const int rr = k / (TX / 4), cc = k % (TX / 4);
-        if (rowout & (1 << (rr >> 2))) {
+        const int y = y0 + rr, x = x0 + 4 * cc;
+        if ((rowout & (1 << (rr >> 2))) && !(a.inplace && (y >= a.H || x >= a.W))) {
           const float4 val = *reinterpret_cast<const float4 *>(&sW[(rr + 1) * SP + PADL + 4 * cc]);
-          __stcg(reinterpret_cast<float4 *>(a.Wp + (size_t)(y0 + 1 + rr) * a.pitch + (x0 + PADL)) + cc, val);
+          __stcg(reinterpret_cast<float4 *>(a.Wp + (size_t)(y + a.woy) * a.pitch + x + a.wox), val);
+          // (without TMA the staged round saves its Z here)
+          if (STAGE && !a.use_tma)
+            __stcg(reinterpret_cast<float4 *>(a.zcopy + (size_t)y * a.W + x),
+                   *reinterpret_cast<const float4 *>(&sZ[rr * TX + 4 * cc]));
         }
       }
     }
@@ -509,6 +542,7 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
       }
     }
   }
+  if (STAGE && a.use_tma && tid == 0) bulk_wait_all();  // the Z stores are done before the CTA's shared memory goes
 }
 
 // ---- level-ordered mode: split the round's worklist into admitted / postponed tiles ----------
@@ -600,24 +634,24 @@ __global__ void __launch_bounds__(256) fill_lift_row_kernel(float *row, int W, c
 }
 
 // ---- layout kernels ----------------------------------------------------------------------
-// compact dem (H x W) -> padded Z and W.  Border cells (all four sides of the raster handed in)
-// are boundary conditions: W = Z = dem there; interior W = +inf; padding Z = W = +inf.
+// compact dem (H x W) -> Z and W in a `pitch` x `rows` layout whose cell (x, y) sits at (x + ox, y + oy): the padded
+// pair (PADL, 1), or in place (0, 0; Wo may be `dem` itself, each thread reads its cells before it writes them).  Border
+// cells (all four sides of the raster handed in) are boundary conditions: W = Z = dem there; interior W = +inf; padding
+// Z = W = +inf.
 // LIFT (fill_multigrid): interior cells start at the water level of their pool x pool block in the filled max-pooled
 // raster `coarse` (an upper bound of the answer, see fill_depressions_dev) instead of +inf.
-// Zp may be null: the sweep then reads Z from `dem` itself.
 template <bool LIFT>
-__global__ void fill_init_kernel(const float *__restrict__ dem, float *__restrict__ Zp,
-                                 float *__restrict__ Wp, int W, int H, int pitch, int rows, FillDev *dev,
-                                 const float *__restrict__ coarse, int Wc, int pool, int yoff) {
-  const int px4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;  // padded column (multiple of 4)
+__global__ void fill_init_kernel(const float *dem, float *__restrict__ Zo, float *Wo, int W, int H, int pitch, int rows,
+                                 int ox, int oy, FillDev *dev, const float *__restrict__ coarse, int Wc, int pool, int yoff) {
+  const int px4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;  // layout column (multiple of 4)
   const float inf = __int_as_float(0x7f800000);
   float lo = inf, hi = -inf;
   for (int py = blockIdx.y; py < rows && px4 < pitch; py += gridDim.y) {
     float zv[4], wv[4];
-    const int y = py - 1;
+    const int y = py - oy;
 #pragma unroll
     for (int k = 0; k < 4; k++) {
-      const int x = px4 + k - PADL;
+      const int x = px4 + k - ox;
       float zz = inf, ww = inf;
       if (x >= 0 && x < W && y >= 0 && y < H) {
         zz = dem[(size_t)y * W + x];
@@ -632,8 +666,8 @@ __global__ void fill_init_kernel(const float *__restrict__ dem, float *__restric
       wv[k] = ww;
     }
     const size_t o = (size_t)py * pitch + px4;
-    if (Zp) *reinterpret_cast<float4 *>(Zp + o) = make_float4(zv[0], zv[1], zv[2], zv[3]);
-    *reinterpret_cast<float4 *>(Wp + o) = make_float4(wv[0], wv[1], wv[2], wv[3]);
+    *reinterpret_cast<float4 *>(Zo + o) = make_float4(zv[0], zv[1], zv[2], zv[3]);
+    *reinterpret_cast<float4 *>(Wo + o) = make_float4(wv[0], wv[1], wv[2], wv[3]);
   }
   for (int o = 16; o > 0; o >>= 1) {
     lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, o));
@@ -651,24 +685,6 @@ __global__ void fill_init_kernel(const float *__restrict__ dem, float *__restric
     if (lo <= hi) {
       atomicMin(&dev->zmin_ord, f2ord(lo));
       atomicMax(&dev->zmax_ord, f2ord(hi));
-    }
-  }
-}
-
-// padded W of a staged lifted start: only the padding frame (rows 0 and rows - 1, PADL columns on either side) is +inf
-// here; the first sweep round writes every tile's cells
-__global__ void __launch_bounds__(256) fill_frame_kernel(float *__restrict__ Wp, int pitch, int rows) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const float inf = __int_as_float(0x7f800000);
-  if (i < pitch) {
-    Wp[i] = inf;
-    Wp[(size_t)(rows - 1) * pitch + i] = inf;
-  }
-  if (i < rows) {
-#pragma unroll
-    for (int j = 0; j < PADL; j++) {
-      Wp[(size_t)i * pitch + j] = inf;
-      Wp[(size_t)i * pitch + pitch - PADL + j] = inf;
     }
   }
 }
@@ -772,22 +788,24 @@ __global__ void __launch_bounds__(256) fill_maxpool_kernel(const float *__restri
 
 // V-cycle (fill_vcycle): restriction -- the coarse surface drops to the block maximum of the current fine surface
 // wherever that is lower (both are upper bounds of the answer for every cell of the block) ...
-// The coarse surface is the padded water-level array of the coarse level's own solver (pitch `cpitch`, cell (bx, by) at
-// (by + 1) * cpitch + bx + PADL); coarse tiles that hold a lowered cell -- and their neighbours when the cell sits on a
-// tile edge -- are flagged for that solver's next run.  `dirty` (may be null; used when k divides the tile shape): only
-// blocks inside fine tiles that were written since the last restriction are looked at.
-__global__ void __launch_bounds__(256) fill_restrict_kernel(const float *__restrict__ Wp, int pitch, int W, int H,
-                                                             float *Wc, int cpitch, int Wcw, int Hc, int k,
-                                                             const int *__restrict__ dirty, int tilesX, int *ctile_flag,
-                                                             int ctilesX) {
+// The fine surface's cell (x, y) is at Wp[(y + woy) * pitch + x + wox] (see FillState::Wb).  The coarse surface is the
+// water-level array of the coarse level's own solver (cell (bx, by) at Wc[(by + coy) * cpitch + bx + cox]); coarse tiles
+// that hold a lowered cell -- and their neighbours when the cell sits on a tile edge -- are flagged for that solver's next
+// run.  `dirty` (may be null; used when k divides the tile shape): only blocks inside fine tiles that were written since
+// the last restriction are looked at.
+__global__ void __launch_bounds__(256) fill_restrict_kernel(const float *__restrict__ Wp, int pitch, int wox, int woy, int W,
+                                                             int H, float *Wc, int cpitch, int cox, int coy, int Wcw, int Hc,
+                                                             int k, const int *__restrict__ dirty, int tilesX,
+                                                             int *ctile_flag, int ctilesX) {
   const int bx = blockIdx.x * blockDim.x + threadIdx.x;
   if (bx >= Wcw) return;
   for (int by = blockIdx.y; by < Hc; by += gridDim.y) {
     if (dirty && !dirty[((by * k) / TY) * tilesX + (bx * k) / TX]) continue;
     float m = -__int_as_float(0x7f800000);
-    if ((k & 3) == 0 && bx * k + k <= W && by * k + k <= H) {  // whole block inside the raster: 16-byte loads
+    // whole block inside the raster: 16-byte loads (pitch and wox are multiples of 4 in both layouts)
+    if ((k & 3) == 0 && bx * k + k <= W && by * k + k <= H) {
       for (int j = 0; j < k; j++) {
-        const float4 *row = reinterpret_cast<const float4 *>(Wp + (size_t)(by * k + j + 1) * pitch + bx * k + PADL);
+        const float4 *row = reinterpret_cast<const float4 *>(Wp + (size_t)(by * k + j + woy) * pitch + bx * k + wox);
         for (int i = 0; i < k / 4; i++) {
           const float4 q = __ldcg(row + i);
           m = fmaxf(fmaxf(m, fmaxf(q.x, q.y)), fmaxf(q.z, q.w));
@@ -799,11 +817,11 @@ __global__ void __launch_bounds__(256) fill_restrict_kernel(const float *__restr
         if (y >= H) break;
         for (int i = 0; i < k; i++) {
           const int x = bx * k + i;
-          if (x < W) m = fmaxf(m, __ldcg(Wp + (size_t)(y + 1) * pitch + x + PADL));
+          if (x < W) m = fmaxf(m, __ldcg(Wp + (size_t)(y + woy) * pitch + x + wox));
         }
       }
     }
-    float *o = Wc + (size_t)(by + 1) * cpitch + bx + PADL;
+    float *o = Wc + (size_t)(by + coy) * cpitch + bx + cox;
     if (m < *o && bx > 0 && by > 0 && bx < Wcw - 1 && by < Hc - 1) {  // border blocks stay pinned at their elevation
       *o = m;
       const int ty0 = (by - 1) / TY, ty1 = (by + 1) / TY, tx0 = (bx - 1) / TX, tx1 = (bx + 1) / TX;
@@ -821,7 +839,8 @@ __global__ void __launch_bounds__(256) fill_restrict_kernel(const float *__restr
 // max-combined into the full coarse array `out` (pre-filled with -inf; merged across bands by a MAX all-reduce)
 // `dirty` (may be null; used when k divides the tile shape and the band starts on a block boundary): blocks inside fine
 // tiles that no sweep has written since the last call report +inf, i.e. "leave the coarse level as it is".
-__global__ void __launch_bounds__(256) fill_blockmax_kernel(const float *__restrict__ Wp, int pitch, int W, int y_lo, int y_hi,
+__global__ void __launch_bounds__(256) fill_blockmax_kernel(const float *__restrict__ Wp, int pitch, int wox, int woy, int W,
+                                                             int y_lo, int y_hi,
                                                              int yoff, float *out, int Wcw, int Hc, int k,
                                                              const int *__restrict__ dirty, int tilesX) {
   const int bx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -846,7 +865,7 @@ __global__ void __launch_bounds__(256) fill_blockmax_kernel(const float *__restr
       if (y >= y_hi) break;
       for (int i = 0; i < k; i++) {
         const int x = bx * k + i;
-        if (x < W) m = fmaxf(m, __ldcg(Wp + (size_t)(y + 1) * pitch + x + PADL));
+        if (x < W) m = fmaxf(m, __ldcg(Wp + (size_t)(y + woy) * pitch + x + wox));
       }
     }
     float *o = out + (size_t)by * Wcw + bx;
@@ -856,10 +875,12 @@ __global__ void __launch_bounds__(256) fill_blockmax_kernel(const float *__restr
 
 // ... and prolongation: every interior fine cell drops to its block's (re-relaxed) coarse level where that is lower;
 // the tiles that hold such a cell -- and the neighbouring tiles whose apron it is part of -- are flagged so that the
-// sweep looks at them again.  The coarse surface is read at Wc[(by + coff_y) * cpitch + bx + coff_x] (a compact array:
-// offsets 0; the coarse solver's padded array: 1 and PADL).  One block per fine tile; `cdirty` (may be null): tiles
-// whose blocks all lie in coarse tiles that the coarse relaxation did not write are skipped.
-__global__ void __launch_bounds__(256) fill_prolong_kernel(float *Wp, int pitch, int W, int H, const float *__restrict__ Wc,
+// sweep looks at them again.  The fine surface's cell (x, y) is at Wp[(y + woy) * pitch + x + wox], the coarse one's at
+// Wc[(by + coff_y) * cpitch + bx + coff_x] (a compact array or a solver in place: offsets 0; a padded solver: 1 and
+// PADL).  One block per fine tile; `cdirty` (may be null): tiles whose blocks all lie in coarse tiles that the coarse
+// relaxation did not write are skipped.
+__global__ void __launch_bounds__(256) fill_prolong_kernel(float *Wp, int pitch, int wox, int woy, int W, int H,
+                                                            const float *__restrict__ Wc,
                                                             int cpitch, int coff_x, int coff_y, int k, int *tile_flag,
                                                             int tilesX, int yoff, const int *__restrict__ cdirty,
                                                             int ctilesX) {
@@ -879,8 +900,9 @@ __global__ void __launch_bounds__(256) fill_prolong_kernel(float *Wp, int pitch,
   for (int g = threadIdx.x; g < TX * TY / 4; g += blockDim.x) {  // 4 cells per thread and step (16-byte accesses)
     const int ly = g / (TX / 4), lx4 = (g - ly * (TX / 4)) * 4;
     const int y = y0 + ly;
-    if (y < 1 || y >= H - 1) continue;
-    float4 *wp4 = reinterpret_cast<float4 *>(Wp + (size_t)(y + 1) * pitch + x0 + lx4 + PADL);
+    // (in place W % 4 == 0: the 4 cells lie wholly inside or wholly outside the raster)
+    if (y < 1 || y >= H - 1 || x0 + lx4 >= W) continue;
+    float4 *wp4 = reinterpret_cast<float4 *>(Wp + (size_t)(y + woy) * pitch + x0 + lx4 + wox);
     const float4 w4 = *wp4;
     float wv[4] = {w4.x, w4.y, w4.z, w4.w};
     const float *crow = Wc + (size_t)((y + yoff) / k + coff_y) * cpitch + coff_x;
@@ -920,22 +942,23 @@ __global__ void __launch_bounds__(256) fill_prolong_kernel(float *Wp, int pitch,
   }
 }
 
-// W % 4 == 0 version: 16-byte loads and stores (padded rows start 16-byte aligned at column PADL)
+// W (cell (x, y) at Wp[(y + woy) * pitch + x + wox]) -> the caller's compact raster.  W % 4 == 0 version: 16-byte loads
+// and stores (rows start 16-byte aligned at column wox)
 __global__ void __launch_bounds__(256) fill_finish_x4_kernel(const float *__restrict__ Wp, float *__restrict__ out, int W,
-                                                              int H, int pitch) {
+                                                              int H, int pitch, int wox, int woy) {
   const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
   if (x4 >= W) return;
   for (int y = blockIdx.y; y < H; y += gridDim.y) {
-    const float4 v = __ldcs(reinterpret_cast<const float4 *>(Wp + (size_t)(y + 1) * pitch + x4 + PADL));
+    const float4 v = __ldcs(reinterpret_cast<const float4 *>(Wp + (size_t)(y + woy) * pitch + x4 + wox));
     __stcs(reinterpret_cast<float4 *>(out + (size_t)y * W + x4), v);
   }
 }
 
 __global__ void fill_finish_kernel(const float *__restrict__ Wp, float *__restrict__ out, int W, int H,
-                                   int pitch) {
+                                   int pitch, int wox, int woy) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x;
   if (x >= W) return;
-  for (int y = blockIdx.y; y < H; y += gridDim.y) out[(size_t)y * W + x] = Wp[(size_t)(y + 1) * pitch + x + PADL];
+  for (int y = blockIdx.y; y < H; y += gridDim.y) out[(size_t)y * W + x] = Wp[(size_t)(y + woy) * pitch + x + wox];
 }
 
 // ---- host side ---------------------------------------------------------------------------
@@ -993,17 +1016,35 @@ struct FillState {
   bool still_active = false;
   int64_t sched_round = 0;
 
-  // Z read straight from the caller's raster (no padded copy; see begin's `dem_stays`)
-  const float *zext = nullptr;
-  // staged lifted start: the first sweep round builds W from this coarse surface (see fill_sweep_kernel)
+  // Where W lives: cell (x, y) at Wb[(y + woy) * wpitch + x + wox].  Padded layout: Wp (pitch, PADL, 1), with Z in Zp.
+  // In place: the caller's raster (W, 0, 0), with Z in the compact copy Zc.
+  float *Wb = nullptr;
+  int wpitch = 0, wox = 0, woy = 0;
+  bool inplace = false;
+  DevBuf<float> Zc;
+  // staged lifted start: the first sweep round builds W from this coarse surface, reads Z from the caller's raster and
+  // saves it to Zc (see fill_sweep_kernel)
   const float *stage_coarse = nullptr;
   int stage_wc = 0, stage_k = 1, stage_yoff = 0;
+  CUtensorMap mapZstage;  // the caller's raster as Z (staged round)
 
-  // dem_stays: d_dem is left as it is until finish() (and the state uses no row updates), so the sweep may read Z from
-  // it instead of a padded copy.  It does so when TMA can address the raster: width a multiple of 4, 16-byte aligned.
-  // With a lifted start, that also lets the first round build its W from the coarse surface (no W pass beforehand).
+  void use_padded_layout(size_t np) {
+    inplace = false;
+    Zc.reset();
+    Zp.alloc(np);
+    Wp.alloc(np);
+    Wb = Wp.p;
+    wpitch = pitch;
+    wox = PADL;
+    woy = 1;
+  }
+
+  // in_place: the caller hands its raster over for the whole solve (no row updates): W is relaxed in it, Z is kept in a
+  // compact copy.  Taken when TMA can address the raster: width a multiple of 4, 16-byte aligned (fill_external_z = 0
+  // turns it off).  With a lifted start the first round then builds its W from the coarse surface and saves Z as it goes
+  // (no pass over the raster beforehand); otherwise the padded layout holds a copy of both.
   void begin(const float *d_dem, int w, int h, const float *d_coarse = nullptr, int coarse_w = 0, int coarse_k = 0,
-             int coarse_yoff = 0, bool dem_stays = false) {
+             int coarse_yoff = 0, bool in_place = false) {
     Ctx &c = ctx();
     W = w;
     H = h;
@@ -1012,14 +1053,21 @@ struct FillState {
     pitch = tilesX * TX + 2 * PADL;
     rows = tilesY * TY + 2;
     const size_t np = (size_t)pitch * rows;
-    zext = dem_stays && c.params.fill_external_z != 0 && (w & 3) == 0 && ((uintptr_t)d_dem & 15) == 0 ? d_dem : nullptr;
-    stage_coarse = zext && d_coarse ? d_coarse : nullptr;
+    if (in_place && c.params.fill_external_z != 0 && (w & 3) == 0 && ((uintptr_t)d_dem & 15) == 0) {
+      inplace = true;
+      Zp.reset();
+      Wp.reset();
+      Zc.alloc((size_t)w * h);
+      Wb = const_cast<float *>(d_dem);  // (in_place: the caller's raster is writable)
+      wpitch = w;
+      wox = woy = 0;
+    } else {
+      use_padded_layout(np);
+    }
+    stage_coarse = inplace && d_coarse ? d_coarse : nullptr;
     stage_wc = coarse_w;
     stage_k = coarse_k;
     stage_yoff = coarse_yoff;
-    if (zext) Zp.reset();
-    else Zp.alloc(np);
-    Wp.alloc(np);
     const size_t nt = (size_t)tilesX * tilesY;
     list0.alloc(nt);
     list1.alloc(nt);
@@ -1047,20 +1095,25 @@ struct FillState {
     {
       const int n2 = (int)(2 * nt);
       fill_i32_kernel<<<(n2 + 255) / 256, 256, 0, c.stream>>>(keys.p, ORD_POS_INF, n2);
+      count_launch();
       dim3 blk(128), grd((pitch / 4 + 127) / 128, rows < 2048 ? rows : 2048);
       if (stage_coarse) {
-        // the first round writes every tile's cells; only the frame is left (zmin / zmax serve the level schedule,
-        // which a lifted start does not use)
-        const int n = pitch > rows ? pitch : rows;
-        fill_frame_kernel<<<(n + 255) / 256, 256, 0, c.stream>>>(Wp.p, pitch, rows);
+        // nothing to do: the first round writes every tile's cells (zmin / zmax serve the level schedule, which a lifted
+        // start does not use)
+      } else if (inplace) {
+        dim3 grdc((W / 4 + 127) / 128, H < 2048 ? H : 2048);
+        fill_init_kernel<false><<<grdc, blk, 0, c.stream>>>(d_dem, Zc.p, Wb, W, H, W, H, 0, 0, dev.p, nullptr, 0, 1, 0);
+        count_launch();
       } else if (d_coarse) {
-        fill_init_kernel<true><<<grd, blk, 0, c.stream>>>(d_dem, Zp.p, Wp.p, W, H, pitch, rows, dev.p, d_coarse, coarse_w, coarse_k,
-                                                         coarse_yoff);
+        fill_init_kernel<true><<<grd, blk, 0, c.stream>>>(d_dem, Zp.p, Wp.p, W, H, pitch, rows, PADL, 1, dev.p, d_coarse,
+                                                         coarse_w, coarse_k, coarse_yoff);
+        count_launch();
       } else {
-        fill_init_kernel<false><<<grd, blk, 0, c.stream>>>(d_dem, Zp.p, Wp.p, W, H, pitch, rows, dev.p, nullptr, 0, 1, 0);
+        fill_init_kernel<false><<<grd, blk, 0, c.stream>>>(d_dem, Zp.p, Wp.p, W, H, pitch, rows, PADL, 1, dev.p, nullptr, 0, 1,
+                                                          0);
+        count_launch();
       }
       RDB_CK(cudaGetLastError());
-      count_launch(2);
       zmin = zmax = 0.f;
       if (!d_coarse) {
         FillDev *hd = (FillDev *)c.pinned;
@@ -1086,8 +1139,8 @@ struct FillState {
           const int stride = rows > 4096 ? 16 : (rows > 512 ? 4 : 1);
           const int nb = (rows - 2 + stride - 1) / stride;
           // (padded rows 1, 1 + stride, ... are raster rows 0, stride, ...)
-          if (zext)
-            fill_hist_kernel<<<nb, 256, 0, c.stream>>>(zext, W, W, H, stride, zmin, 1.0f / (zmax - zmin), hist.p);
+          if (inplace)  // (the caller's raster holds W by now)
+            fill_hist_kernel<<<nb, 256, 0, c.stream>>>(Zc.p, W, W, H, stride, zmin, 1.0f / (zmax - zmin), hist.p);
           else
             fill_hist_kernel<<<nb, 256, 0, c.stream>>>(Zp.p + pitch, pitch, pitch, rows - 1, stride, zmin, 1.0f / (zmax - zmin),
                                                        hist.p);
@@ -1109,9 +1162,15 @@ struct FillState {
         }
       }
     }
-    mapW = make_map(Wp.p, pitch, rows, SP, SROWS);
-    // (TMA fills the box cells beyond the raster's edge with zeros; the sweep overwrites them with +inf)
-    mapZ = zext ? make_map(const_cast<float *>(zext), W, H, TX, TY) : make_map(Zp.p, pitch, rows, TX, TY);
+    if (inplace) {
+      // (TMA fills the box cells beyond the raster's edges with zeros; the sweep overwrites them with +inf)
+      mapW = make_map(Wb, W, H, SP, SROWS);
+      mapZ = make_map(Zc.p, W, H, TX, TY);
+      if (stage_coarse) mapZstage = make_map(Wb, W, H, TX, TY);
+    } else {
+      mapW = make_map(Wp.p, pitch, rows, SP, SROWS);
+      mapZ = make_map(Zp.p, pitch, rows, TX, TY);
+    }
     int per_sm = 0;
     RDB_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fill_sweep_kernel<0>, FILL_THREADS, 0));
     if (per_sm < 1) per_sm = 1;
@@ -1138,9 +1197,7 @@ struct FillState {
     tilesY = (h + TY - 1) / TY;
     pitch = tilesX * TX + 2 * PADL;
     rows = tilesY * TY + 2;
-    const size_t np = (size_t)pitch * rows;
-    Zp.alloc(np);
-    Wp.alloc(np);
+    use_padded_layout((size_t)pitch * rows);
     const size_t nt = (size_t)tilesX * tilesY;
     list0.alloc(nt);
     list1.alloc(nt);
@@ -1190,10 +1247,10 @@ struct FillState {
     Ctx &c = ctx();
     FillArgs a;
     memset(&a, 0, sizeof(a));
-    if (zext) {
-      a.Z = zext;
+    if (inplace) {
+      a.Z = Zc.p;
       a.zpitch = W;
-      a.zext = 1;
+      a.inplace = 1;
     } else {
       a.Z = Zp.p;
       a.zpitch = pitch;
@@ -1204,8 +1261,10 @@ struct FillState {
     a.pool = stage_k;
     a.yoff = stage_yoff;
     a.staged = staged.p;
-    a.Wp = Wp.p;
-    a.pitch = pitch;
+    a.Wp = Wb;
+    a.pitch = wpitch;
+    a.wox = wox;
+    a.woy = woy;
     a.W = W;
     a.H = H;
     a.tilesX = tilesX;
@@ -1246,13 +1305,17 @@ struct FillState {
         a.use_proc = 0;
       }
       sched_round++;
-      // round 1 of a staged lifted start visits every tile (seeded in begin) and builds W instead of loading it
+      // round 1 of a staged lifted start visits every tile (seeded in begin) and builds W instead of loading it; Z is
+      // still the caller's raster then, and every tile saves it to Zc (mapZ) before it writes its W
       a.coarse = round == 1 ? stage_coarse : nullptr;
-      if (step_mode) fill_sweep_kernel<1><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mapZ, a);
-      else if (a.coarse && topo4) fill_sweep_kernel<0, true, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mapZ, a);
-      else if (a.coarse) fill_sweep_kernel<0, false, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mapZ, a);
-      else if (topo4) fill_sweep_kernel<0, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mapZ, a);
-      else fill_sweep_kernel<0><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mapZ, a);
+      a.Z = a.coarse ? Wb : (inplace ? Zc.p : Zp.p);
+      a.zcopy = a.coarse ? Zc.p : nullptr;
+      const CUtensorMap &mz = a.coarse ? mapZstage : mapZ;
+      if (step_mode) fill_sweep_kernel<1><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mz, mapZ, a);
+      else if (a.coarse && topo4) fill_sweep_kernel<0, true, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mz, mapZ, a);
+      else if (a.coarse) fill_sweep_kernel<0, false, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mz, mapZ, a);
+      else if (topo4) fill_sweep_kernel<0, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mz, mapZ, a);
+      else fill_sweep_kernel<0><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mz, mapZ, a);
       round++;
     }
     if (timed) RDB_CK(cudaEventRecord(c.evk1, c.stream));
@@ -1337,15 +1400,15 @@ struct FillState {
     if (!tflag.p) tflag.alloc(nt);
     RDB_CK(cudaMemsetAsync(tflag.p, 0, nt * sizeof(int), ctx().stream));
   }
-  // restriction of THIS (fine) level's surface into the coarse level's solver `cs` (its padded water levels drop to the
+  // restriction of THIS (fine) level's surface into the coarse level's solver `cs` (its water levels drop to the
   // k x k block maxima where those are lower; the coarse tiles touched are queued for cs's next run)
   void restrict_into(FillState &cs, int k) {
     Ctx &c = ctx();
     cs.clear_flags();
     const bool selective = dirty.p && TX % k == 0 && TY % k == 0;
     dim3 blk(256), grd((unsigned)((cs.W + 255) / 256), (unsigned)(cs.H < 4096 ? cs.H : 4096));
-    fill_restrict_kernel<<<grd, blk, 0, c.stream>>>(Wp.p, pitch, W, H, cs.Wp.p, cs.pitch, cs.W, cs.H, k,
-                                                    selective ? dirty.p : nullptr, tilesX, cs.tflag.p, cs.tilesX);
+    fill_restrict_kernel<<<grd, blk, 0, c.stream>>>(Wb, wpitch, wox, woy, W, H, cs.Wb, cs.wpitch, cs.wox, cs.woy, cs.W, cs.H,
+                                                    k, selective ? dirty.p : nullptr, tilesX, cs.tflag.p, cs.tilesX);
     RDB_CK(cudaGetLastError());
     count_launch();
     cs.seed_from_flags();
@@ -1357,7 +1420,8 @@ struct FillState {
     Ctx &c = ctx();
     dim3 blk(256), grd((unsigned)((wc + 255) / 256), (unsigned)((y_hi - y_lo) / k + 2 < 4096 ? (y_hi - y_lo) / k + 2 : 4096));
     const bool sel = selective && dirty.p && TX % k == 0;  // (columns of a block then lie in one tile column)
-    fill_blockmax_kernel<<<grd, blk, 0, c.stream>>>(Wp.p, pitch, W, y_lo, y_hi, yoff, d_out, wc, hc, k, sel ? dirty.p : nullptr, tilesX);
+    fill_blockmax_kernel<<<grd, blk, 0, c.stream>>>(Wb, wpitch, wox, woy, W, y_lo, y_hi, yoff, d_out, wc, hc, k,
+                                                    sel ? dirty.p : nullptr, tilesX);
     RDB_CK(cudaGetLastError());
     count_launch();
     if (sel) clear_dirty();
@@ -1370,14 +1434,14 @@ struct FillState {
     Ctx &c = ctx();
     clear_flags();
     const int nt = tilesX * tilesY;
-    fill_prolong_kernel<<<nt, 256, 0, c.stream>>>(Wp.p, pitch, W, H, d_wc, cpitch, coff_x, coff_y, k, tflag.p, tilesX, yoff,
-                                                  cdirty, ctilesX);
+    fill_prolong_kernel<<<nt, 256, 0, c.stream>>>(Wb, wpitch, wox, woy, W, H, d_wc, cpitch, coff_x, coff_y, k, tflag.p, tilesX,
+                                                  yoff, cdirty, ctilesX);
     RDB_CK(cudaGetLastError());
     count_launch();
     seed_from_flags(d_count);
   }
   void prolong_from_level(FillState &cs, int k, int yoff = 0, int *d_count = nullptr) {
-    prolong_from(cs.Wp.p, cs.pitch, PADL, 1, k, yoff, cs.dirty.p, cs.tilesX, d_count);
+    prolong_from(cs.Wb, cs.wpitch, cs.wox, cs.woy, k, yoff, cs.dirty.p, cs.tilesX, d_count);
     cs.clear_dirty();
   }
   // a neighbouring band's edge row arrives: ghost row y (0 or H-1) drops to it where it is lower; the tiles that read
@@ -1393,10 +1457,11 @@ struct FillState {
 
   void read_row(int y, float *d_row) {
     if (y < 0 || y >= H) fail("fill_read_row: row %d out of range", y);
-    RDB_CK(cudaMemcpyAsync(d_row, Wp.p + (size_t)(y + 1) * pitch + PADL, (size_t)W * 4,
+    RDB_CK(cudaMemcpyAsync(d_row, Wb + (size_t)(y + woy) * wpitch + wox, (size_t)W * 4,
                            cudaMemcpyDeviceToDevice, ctx().stream));
   }
 
+  // (row-band states only: they keep the padded layout)
   void update_row(int y, const float *d_row) {
     if (y != 0 && y != H - 1) fail("fill_update_row: only boundary rows (0, height-1) can be replaced");
     Ctx &c = ctx();
@@ -1432,12 +1497,13 @@ struct FillState {
 
   void finish(float *d_out) {
     Ctx &c = ctx();
+    if (d_out == Wb) return;  // in place: the answer is where it belongs already
     if ((W & 3) == 0 && ((uintptr_t)d_out & 15) == 0) {
       dim3 blk(256), grd((W / 4 + 255) / 256, H < 4096 ? H : 4096);
-      fill_finish_x4_kernel<<<grd, blk, 0, c.stream>>>(Wp.p, d_out, W, H, pitch);
+      fill_finish_x4_kernel<<<grd, blk, 0, c.stream>>>(Wb, d_out, W, H, wpitch, wox, woy);
     } else {
       dim3 blk(256), grd((W + 255) / 256, H < 32768 ? H : 32768);
-      fill_finish_kernel<<<grd, blk, 0, c.stream>>>(Wp.p, d_out, W, H, pitch);
+      fill_finish_kernel<<<grd, blk, 0, c.stream>>>(Wb, d_out, W, H, wpitch, wox, woy);
     }
     RDB_CK(cudaGetLastError());
     count_launch();
@@ -1564,7 +1630,8 @@ static void fill_depressions_level(float *d_dem, int w, int h, int depth, bool t
     extra.fill_rounds -= before.fill_rounds;
     extra.fill_tile_visits -= before.fill_tile_visits;
     extra.fill_tile_iters -= before.fill_tile_iters;
-    // (d_dem, zc and coarse stay as they are until st.finish: the solvers read Z, and round 1 its start, from them)
+    // (both solvers run in place where they can: st relaxes W in d_dem, cst in zc, which nothing else reads; `coarse`
+    // stays as it is until both are done: their first rounds build their start from it)
     st.begin(d_dem, w, h, coarse.p, wc, k, 0, true);
     if (every <= 0) {
       st.run();
@@ -1575,7 +1642,7 @@ static void fill_depressions_level(float *d_dem, int w, int h, int depth, bool t
       // and handed back (prolongation: fine = min(fine, lifted)).  Restriction and coarse relaxation keep every coarse
       // value an upper bound of the answer for all cells of its block, so the fine surface stays an upper bound and
       // still relaxes to exactly W*.
-      // The coarse level keeps ONE solver for all corrections (cst): restriction lowers its padded surface in place
+      // The coarse level keeps ONE solver for all corrections (cst): restriction lowers its surface in place
       // and queues the coarse tiles it touched, its relaxation notes the tiles it writes, and the prolongation only
       // looks at the fine tiles below those -- a correction costs what it changes, not three passes over the raster.
       FillState cst;
