@@ -94,6 +94,21 @@ RDB200_API int rdb200_fill_depressions_d8_f32(float *dem, int32_t width, int32_t
  *   Same engine with the 4-neighbour stencil; bit-identical. */
 RDB200_API int rdb200_fill_depressions_d4_f32(float *dem, int32_t width, int32_t height);
 
+/* richdem::pit_mask<Topology::D8 / D4>(const Array2D<float>&, Array2D<uint8_t>&)
+ *   include/richdem/depressions/Barnes2014.hpp:593-676 (app rd_depressions_mask).  mask (width x height, written in
+ *   full): 3 where dem == nodata, 1 where the cell lies below the depression-filled surface of dem (the fill above,
+ *   NoData an ordinary value), 0 elsewhere -- edge cells and cells at their filled level included, which the reference
+ *   leaves as its resize() set them.  dem is not modified.  Bit-identical. */
+RDB200_API int rdb200_pit_mask_d8_f32(const float *dem, uint8_t *mask, int32_t width, int32_t height, float nodata);
+RDB200_API int rdb200_pit_mask_d4_f32(const float *dem, uint8_t *mask, int32_t width, int32_t height, float nodata);
+
+/* richdem::HasDepressions<Topology::D8 / D4>(const Array2D<float>&)
+ *   include/richdem/depressions/Barnes2014.hpp:43-104 (app rd_depressions_has).  *out = 1 if some cell lies below the
+ *   filled surface, else 0 (NoData is not special, as in the reference).  A stencil pass that finds a strict pit answers
+ *   without filling. */
+RDB200_API int rdb200_has_depressions_d8_f32(const float *dem, int32_t width, int32_t height, int32_t *out);
+RDB200_API int rdb200_has_depressions_d4_f32(const float *dem, int32_t width, int32_t height, int32_t *out);
+
 /* richdem::ResolveFlatsEpsilon(Array2D<float>&)
  *   include/richdem/flats/flats.hpp:21-28 (GetFlatMask + ResolveFlatsEpsilon_Barnes2014,
  *   include/richdem/flats/Barnes2014.hpp:398-467, 496-550); pyrichdem rdResolveFlatsEpsilon
@@ -211,6 +226,11 @@ RDB200_API int rdb200_fa_tarboton_f32_f64(const float *dem, double *accum_inout,
  * d_dem are unspecified. */
 RDB200_API int rdb200_dev_fill_depressions_d8_f32(float *d_dem, int32_t width, int32_t height);
 RDB200_API int rdb200_dev_fill_depressions_d4_f32(float *d_dem, int32_t width, int32_t height);
+/* pit_mask / HasDepressions on device pointers (d_dem is not modified; *out is a host int) */
+RDB200_API int rdb200_dev_pit_mask_d8_f32(const float *d_dem, uint8_t *d_mask, int32_t width, int32_t height, float nodata);
+RDB200_API int rdb200_dev_pit_mask_d4_f32(const float *d_dem, uint8_t *d_mask, int32_t width, int32_t height, float nodata);
+RDB200_API int rdb200_dev_has_depressions_d8_f32(const float *d_dem, int32_t width, int32_t height, int32_t *out);
+RDB200_API int rdb200_dev_has_depressions_d4_f32(const float *d_dem, int32_t width, int32_t height, int32_t *out);
 RDB200_API int rdb200_dev_resolve_flats_epsilon_f32(float *d_dem, int32_t width, int32_t height, float nodata);
 RDB200_API int rdb200_dev_d8_flow_directions_f32(const float *d_dem, uint8_t *d_flowdirs, int32_t width,
                                       int32_t height, float nodata);
@@ -293,6 +313,27 @@ RDB200_API int rdb200_mgpu_fill_depressions_d8_f32(const rdb200_comm *comm, floa
 RDB200_API int rdb200_mgpu_fill_depressions_d4_f32(const rdb200_comm *comm, float *d_band, int32_t width, int32_t local_rows,
                                                    int32_t ghost_top, int32_t ghost_bottom, int32_t row0, int32_t height,
                                                    int32_t *exchange_rounds);
+/* pit_mask<D8 / D4> over row bands.  d_band (local_rows x width, row0 and height as in the band fill) is not modified; its
+ * ghost rows are not read.  The band fill runs on a copy of it, then the owned rows of d_band_mask (local_rows x width)
+ * receive the single-GPU mask, bit for bit; its ghost rows are not written.  The band must own a row, have the ghost
+ * rows its rank needs, and -- when the raster has interior cells -- hold at least three local rows, as the band fill
+ * requires; these are checked before any communication. */
+RDB200_API int rdb200_mgpu_pit_mask_d8_f32(const rdb200_comm *comm, const float *d_band, uint8_t *d_band_mask, int32_t width,
+                                           int32_t local_rows, float nodata, int32_t ghost_top, int32_t ghost_bottom, int32_t row0,
+                                           int32_t height);
+RDB200_API int rdb200_mgpu_pit_mask_d4_f32(const rdb200_comm *comm, const float *d_band, uint8_t *d_band_mask, int32_t width,
+                                           int32_t local_rows, float nodata, int32_t ghost_top, int32_t ghost_bottom, int32_t row0,
+                                           int32_t height);
+/* HasDepressions<D8 / D4> over row bands, arguments as rdb200_mgpu_pit_mask_*.  Every rank first looks for a strict pit
+ * in its owned rows (on a copy whose ghost rows receive the neighbours' edge rows) and one OR all-reduce combines the
+ * answers; the band fill and a second all-reduce run only if no rank found one.  *out (host): 1 or 0 on every rank, the
+ * single-GPU answer. */
+RDB200_API int rdb200_mgpu_has_depressions_d8_f32(const rdb200_comm *comm, const float *d_band, int32_t width, int32_t local_rows,
+                                                  int32_t ghost_top, int32_t ghost_bottom, int32_t row0, int32_t height,
+                                                  int32_t *out);
+RDB200_API int rdb200_mgpu_has_depressions_d4_f32(const rdb200_comm *comm, const float *d_band, int32_t width, int32_t local_rows,
+                                                  int32_t ghost_top, int32_t ghost_bottom, int32_t row0, int32_t height,
+                                                  int32_t *out);
 /* ResolveFlatsEpsilon (include/richdem/flats/flats.hpp:21-28) over row bands, in place on the owned rows of `d_band`
  * (local_rows x width; the ghost rows must hold the neighbours' edge rows on entry, as the fill leaves them, and hold
  * the neighbours' resolved edge rows on return, ready for rdb200_mgpu_fa_*).  Same result as the single-GPU call, bit for

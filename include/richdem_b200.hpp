@@ -161,6 +161,38 @@ inline void PriorityFlood_Zhou2016<float>(Array2D<float> &dem) {
 #endif
 
 #if 1
+// depressions/Barnes2014.hpp:593-676: the output is resized as the reference does (every cell 0) and gets NoData 3; the
+// call then writes every cell, and the ones the reference never writes come out 0 as they do there
+template <>
+inline void pit_mask<Topology::D8, float>(const Array2D<float> &elevations, Array2D<uint8_t> &mask) {
+  mask.resize(elevations.width(), elevations.height());
+  mask.setNoData(3);
+  richdem_b200::check(rdb200_pit_mask_d8_f32(elevations.data(), mask.data(), elevations.width(), elevations.height(),
+                                             elevations.noData()));
+}
+template <>
+inline void pit_mask<Topology::D4, float>(const Array2D<float> &elevations, Array2D<uint8_t> &mask) {
+  mask.resize(elevations.width(), elevations.height());
+  mask.setNoData(3);
+  richdem_b200::check(rdb200_pit_mask_d4_f32(elevations.data(), mask.data(), elevations.width(), elevations.height(),
+                                             elevations.noData()));
+}
+// depressions/Barnes2014.hpp:43-104
+template <>
+inline bool HasDepressions<Topology::D8, float>(const Array2D<float> &elevations) {
+  int32_t any = 0;
+  richdem_b200::check(rdb200_has_depressions_d8_f32(elevations.data(), elevations.width(), elevations.height(), &any));
+  return any != 0;
+}
+template <>
+inline bool HasDepressions<Topology::D4, float>(const Array2D<float> &elevations) {
+  int32_t any = 0;
+  richdem_b200::check(rdb200_has_depressions_d4_f32(elevations.data(), elevations.width(), elevations.height(), &any));
+  return any != 0;
+}
+#endif
+
+#if 1
 // flats/flats.hpp:21-28
 template <>
 inline void ResolveFlatsEpsilon<float>(Array2D<float> &elevations) {

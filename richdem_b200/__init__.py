@@ -12,6 +12,7 @@ fallback and methods outside the hot path raise.
 from __future__ import annotations
 
 import copy
+import ctypes as C
 import datetime
 from typing import Any, Optional
 
@@ -139,6 +140,39 @@ def FillDepressions(dem: rdarray, epsilon: bool = False, in_place: bool = False,
     if not in_place:
         return dem
     return None
+
+
+def PitMask(dem: rdarray, topology: str = "D8") -> rdarray:
+    """richdem::pit_mask<topo> (depressions/Barnes2014.hpp:593-676; app rd_depressions_mask): uint8 mask of the cells
+    that lie in a depression, i.e. below the ``FillDepressions`` surface of ``dem`` (1), NoData cells (3) and all others
+    (0), with ``no_data`` 3 and the input's metadata.  ``dem`` is not modified."""
+    if type(dem) is not rdarray:
+        raise Exception("A richdem.rdarray or numpy.ndarray is required!")
+    if topology not in ["D8", "D4"]:
+        raise Exception("Unknown topology!")
+    d = _dem_f32(dem, "PitMask")
+    h, w = d.shape
+    out = rdarray(np.empty((h, w), np.uint8), meta_obj=dem, no_data=3)
+    _add_analysis(out, f"PitMask(dem, topology={topology})")
+    fn = _lib.lib().rdb200_pit_mask_d8_f32 if topology == "D8" else _lib.lib().rdb200_pit_mask_d4_f32
+    _lib.check(fn(_lib.ptr(d), _lib.ptr(out), w, h, _nodata_f32(dem)))
+    out.no_data = 3
+    return out
+
+
+def HasDepressions(dem: rdarray, topology: str = "D8") -> bool:
+    """richdem::HasDepressions<topo> (depressions/Barnes2014.hpp:43-104; app rd_depressions_has): whether
+    ``FillDepressions`` would raise any cell.  NoData is not special, as in the reference."""
+    if type(dem) is not rdarray:
+        raise Exception("A richdem.rdarray or numpy.ndarray is required!")
+    if topology not in ["D8", "D4"]:
+        raise Exception("Unknown topology!")
+    d = _dem_f32(dem, "HasDepressions")
+    h, w = d.shape
+    out = C.c_int32(0)
+    fn = _lib.lib().rdb200_has_depressions_d8_f32 if topology == "D8" else _lib.lib().rdb200_has_depressions_d4_f32
+    _lib.check(fn(_lib.ptr(d), w, h, C.byref(out)))
+    return bool(out.value)
 
 
 def ResolveFlats(dem: rdarray, in_place: bool = False) -> Optional[rdarray]:

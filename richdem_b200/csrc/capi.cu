@@ -311,6 +311,47 @@ int rdb200_fill_depressions_d4_f32(float *dem, int32_t w, int32_t h) {
   CAPI_END
 }
 
+static int pit_mask_host(const float *dem, uint8_t *mask, int32_t w, int32_t h, float nodata, bool topo4) {
+  CAPI_TRY
+  if (!dem || !mask) fail("pit_mask: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<float> d(n);
+  DevBuf<uint8_t> m(n);
+  h2d(d.p, dem, n);
+  pit_mask_dev(d.p, m.p, w, h, nodata, topo4);
+  d2h(mask, m.p, n);
+  cs.done();
+  CAPI_END
+}
+int rdb200_pit_mask_d8_f32(const float *dem, uint8_t *mask, int32_t w, int32_t h, float nodata) {
+  return pit_mask_host(dem, mask, w, h, nodata, false);
+}
+int rdb200_pit_mask_d4_f32(const float *dem, uint8_t *mask, int32_t w, int32_t h, float nodata) {
+  return pit_mask_host(dem, mask, w, h, nodata, true);
+}
+
+static int has_depressions_host(const float *dem, int32_t w, int32_t h, int32_t *out, bool topo4) {
+  CAPI_TRY
+  if (!dem || !out) fail("has_depressions: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<float> d(n);
+  h2d(d.p, dem, n);
+  const bool any = has_depressions_dev(d.p, w, h, topo4);
+  cs.done();
+  *out = any ? 1 : 0;
+  CAPI_END
+}
+int rdb200_has_depressions_d8_f32(const float *dem, int32_t w, int32_t h, int32_t *out) {
+  return has_depressions_host(dem, w, h, out, false);
+}
+int rdb200_has_depressions_d4_f32(const float *dem, int32_t w, int32_t h, int32_t *out) {
+  return has_depressions_host(dem, w, h, out, true);
+}
+
 int rdb200_resolve_flats_epsilon_f32(float *dem, int32_t w, int32_t h, float nodata) {
   CAPI_TRY
   if (!dem) fail("resolve_flats: null dem");
@@ -538,6 +579,37 @@ int rdb200_dev_fill_depressions_d8_f32(float *d_dem, int32_t w, int32_t h) {
 int rdb200_dev_fill_depressions_d4_f32(float *d_dem, int32_t w, int32_t h) {
   DEV_ENTRY((int64_t)w * h, (check_dims(w, h), fill_depressions_dev(d_dem, w, h, true)))
 }
+static int dev_pit_mask(const float *d_dem, uint8_t *d_mask, int32_t w, int32_t h, float nodata, bool topo4) {
+  CAPI_TRY
+  if (!d_dem || !d_mask) fail("pit_mask: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  pit_mask_dev(d_dem, d_mask, w, h, nodata, topo4);
+  cs.done();
+  CAPI_END
+}
+int rdb200_dev_pit_mask_d8_f32(const float *d_dem, uint8_t *d_mask, int32_t w, int32_t h, float nodata) {
+  return dev_pit_mask(d_dem, d_mask, w, h, nodata, false);
+}
+int rdb200_dev_pit_mask_d4_f32(const float *d_dem, uint8_t *d_mask, int32_t w, int32_t h, float nodata) {
+  return dev_pit_mask(d_dem, d_mask, w, h, nodata, true);
+}
+static int dev_has_depressions(const float *d_dem, int32_t w, int32_t h, int32_t *out, bool topo4) {
+  CAPI_TRY
+  if (!d_dem || !out) fail("has_depressions: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const bool any = has_depressions_dev(d_dem, w, h, topo4);
+  cs.done();
+  *out = any ? 1 : 0;
+  CAPI_END
+}
+int rdb200_dev_has_depressions_d8_f32(const float *d_dem, int32_t w, int32_t h, int32_t *out) {
+  return dev_has_depressions(d_dem, w, h, out, false);
+}
+int rdb200_dev_has_depressions_d4_f32(const float *d_dem, int32_t w, int32_t h, int32_t *out) {
+  return dev_has_depressions(d_dem, w, h, out, true);
+}
 int rdb200_dev_resolve_flats_epsilon_f32(float *d_dem, int32_t w, int32_t h, float nodata) {
   DEV_ENTRY((int64_t)w * h, (check_dims(w, h), resolve_flats_dev(d_dem, w, h, nodata, nullptr, nullptr, true)))
 }
@@ -609,6 +681,43 @@ int rdb200_mgpu_fill_depressions_d4_f32(const rdb200_comm *comm, float *d_band, 
   cs.done();
   if (exchange_rounds) *exchange_rounds = xr;
   CAPI_END
+}
+
+static int mgpu_pit_mask(const rdb200_comm *comm, const float *d_band, uint8_t *d_band_mask, int32_t w, int32_t rows, float nodata,
+                         int32_t gt, int32_t gb, int32_t row0, int32_t height, bool topo4) {
+  CAPI_TRY
+  check_dims(w, rows);
+  CallScope cs((int64_t)w * rows);
+  mgpu_pit_mask_band(comm, d_band, d_band_mask, w, rows, nodata, gt, gb, row0, height, topo4);
+  cs.done();
+  CAPI_END
+}
+int rdb200_mgpu_pit_mask_d8_f32(const rdb200_comm *comm, const float *d_band, uint8_t *d_band_mask, int32_t w, int32_t rows,
+                                float nodata, int32_t gt, int32_t gb, int32_t row0, int32_t height) {
+  return mgpu_pit_mask(comm, d_band, d_band_mask, w, rows, nodata, gt, gb, row0, height, false);
+}
+int rdb200_mgpu_pit_mask_d4_f32(const rdb200_comm *comm, const float *d_band, uint8_t *d_band_mask, int32_t w, int32_t rows,
+                                float nodata, int32_t gt, int32_t gb, int32_t row0, int32_t height) {
+  return mgpu_pit_mask(comm, d_band, d_band_mask, w, rows, nodata, gt, gb, row0, height, true);
+}
+static int mgpu_has_depressions(const rdb200_comm *comm, const float *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb,
+                                int32_t row0, int32_t height, int32_t *out, bool topo4) {
+  CAPI_TRY
+  if (!out) fail("mgpu_has_depressions: null pointer");
+  check_dims(w, rows);
+  CallScope cs((int64_t)w * rows);
+  const bool any = mgpu_has_depressions_band(comm, d_band, w, rows, gt, gb, row0, height, topo4);
+  cs.done();
+  *out = any ? 1 : 0;
+  CAPI_END
+}
+int rdb200_mgpu_has_depressions_d8_f32(const rdb200_comm *comm, const float *d_band, int32_t w, int32_t rows, int32_t gt,
+                                       int32_t gb, int32_t row0, int32_t height, int32_t *out) {
+  return mgpu_has_depressions(comm, d_band, w, rows, gt, gb, row0, height, out, false);
+}
+int rdb200_mgpu_has_depressions_d4_f32(const rdb200_comm *comm, const float *d_band, int32_t w, int32_t rows, int32_t gt,
+                                       int32_t gb, int32_t row0, int32_t height, int32_t *out) {
+  return mgpu_has_depressions(comm, d_band, w, rows, gt, gb, row0, height, out, true);
 }
 
 int rdb200_mgpu_fa_f32_f64(const rdb200_comm *comm, const float *d_dem, double *d_accum, int32_t w, int32_t rows, float nodata,

@@ -204,5 +204,12 @@ void fa_fused_dev(const float *d_dem, double *d_accum, int w, int h, float nodat
 void terrain_attribute_dev(int attribute_id, const float *d_dem, float *d_out, int w, int h, float nodata_in, float nodata_out,
                            float zscale, double cell_x, double cell_y);
 void generate_fbm_dev(float *d_dem, int w, int h, int y0, uint32_t seed, int octaves, float quantum);
+// pit_mask<topo> / HasDepressions<topo> (depressions.cu); d_dem is not modified
+void pit_mask_dev(const float *d_dem, uint8_t *d_mask, int w, int h, float nodata, bool topo4);
+bool has_depressions_dev(const float *d_dem, int w, int h, bool topo4);
+void mgpu_pit_mask_band(const rdb200_comm *comm, const float *d_band, uint8_t *d_mask, int w, int hloc, float nodata, int gt,
+                        int gb, int row0, int H, bool topo4);
+bool mgpu_has_depressions_band(const rdb200_comm *comm, const float *d_band, int w, int hloc, int gt, int gb, int row0, int H,
+                               bool topo4);
 
 }  // namespace rdb

@@ -348,6 +348,60 @@ def fill_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, solver_cls=None
                                rank, world)
 
 
+def _band_geometry(local_dem, g_top, g_bot, row0, height, group):
+    """(row0, height) of a band: as given, or gathered from every rank's owned rows when ``height`` <= 0."""
+    if height > 0:
+        return int(row0), int(height)
+    rank = dist.get_rank(group) if dist.is_initialized() else 0
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    h_ = local_dem.shape[0]
+    if world == 1:
+        return 0, h_
+    hh = torch.tensor([h_ - g_top - g_bot], dtype=torch.int64, device=local_dem.device)
+    allh = [torch.zeros_like(hh) for _ in range(world)]
+    dist.all_gather(allh, hh, group=group)
+    return int(sum(int(t.item()) for t in allh[:rank])) - g_top, int(sum(int(t.item()) for t in allh))
+
+
+def pit_mask_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: float, topology: str = "D8", row0: int = 0,
+                  height: int = 0, group=None) -> "torch.Tensor":
+    """PitMask over this rank's band.  ``local_dem`` is (g_top + owned + g_bot) x W; it is not modified and its ghost rows
+    are not read.  ``row0`` / ``height`` as in :func:`fill_band` (gathered from the ranks when ``height`` <= 0).
+    Collective.  Returns the uint8 mask of the local shape whose owned rows are the single-GPU bits (ghost rows
+    unspecified)."""
+    from . import _lib
+    if topology not in ("D8", "D4"):
+        raise Exception("Unknown topology!")
+    assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
+    row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
+    _lib.use_torch_stream()
+    h, w = local_dem.shape
+    mask = torch.empty((h, w), dtype=torch.uint8, device=local_dem.device)
+    cm = lib_comm(group, local_dem.is_cuda)
+    fn = _lib.lib().rdb200_mgpu_pit_mask_d8_f32 if topology == "D8" else _lib.lib().rdb200_mgpu_pit_mask_d4_f32
+    _lib.check(fn(cm.handle, local_dem.data_ptr(), mask.data_ptr(), w, h, float(nodata), int(g_top), int(g_bot), row0, height))
+    return mask
+
+
+def has_depressions_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, topology: str = "D8", row0: int = 0,
+                         height: int = 0, group=None) -> bool:
+    """HasDepressions of the whole raster, from this rank's band (arguments as :func:`pit_mask_band`).  A strict pit in any
+    band answers after one all-reduce; the band fill runs only when there is none.  Collective; every rank gets the
+    same answer."""
+    from . import _lib
+    if topology not in ("D8", "D4"):
+        raise Exception("Unknown topology!")
+    assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
+    row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
+    _lib.use_torch_stream()
+    h, w = local_dem.shape
+    out = C.c_int32(0)
+    cm = lib_comm(group, local_dem.is_cuda)
+    fn = _lib.lib().rdb200_mgpu_has_depressions_d8_f32 if topology == "D8" else _lib.lib().rdb200_mgpu_has_depressions_d4_f32
+    _lib.check(fn(cm.handle, local_dem.data_ptr(), w, h, int(g_top), int(g_bot), row0, height, C.byref(out)))
+    return bool(out.value)
+
+
 def _fill_band_protocol(local_dem, g_top, g_bot, solver_cls, group, max_rounds, return_stats, multigrid, row0, height, vcycle, rank,
                         world):
     """The Python band protocol behind :func:`fill_band` (RDB_BAND_DRIVER=python and the CPU tests' solvers).  The ghost rows of
