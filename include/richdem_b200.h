@@ -178,6 +178,40 @@ RDB200_API int rdb200_fa_holmgren_f32_f64(const float *dem, double *accum_inout,
 RDB200_API int rdb200_fa_freeman_f32_f64(const float *dem, double *accum_inout, int32_t width, int32_t height,
                                          float nodata, double xparam);
 
+/* float64 elevations: the same reference functions with T = double, bit for bit (the fill's zero sign aside, as for
+ * float).  Each runs the float engine on kappa(dem), a strictly increasing map of the raster's doubles to float keys
+ * (the cast to float when every value is a float already, else dense ranks by a radix sort), and maps the result back;
+ * DESIGN §0 gives the argument.  NaN elevations carry no promise beyond what the float entry points make.
+ *   fill_depressions_*_f64   depressions/depressions.hpp:13-21 -> Zhou2016.hpp:125-191 (D8), Barnes2014.hpp:230-304 (D4);
+ *                            cells the fill does not raise keep their own bits
+ *   pit_mask_*_f64           depressions/Barnes2014.hpp:593-676 (3 NoData, 1 depression, 0 otherwise)
+ *   has_depressions_*_f64    depressions/Barnes2014.hpp:43-104
+ *   resolve_flats_epsilon_f64  flats/flats.hpp:21-28: GetFlatMask (Barnes2014.hpp:398-467) of the keys, then k double
+ *                            ulps (nextafter towards +inf) on the original values (:496-550)
+ *   d8_flow_directions_f64   flowmet/d8_flowdirs.hpp:32-123, compared as doubles
+ *   fa_d8_f64_f64            methods/flow_accumulation.hpp:27 (FA_D8<double, double>); accum_is_ones as rdb200_fa_d8_f32_f64
+ *   fa_d4_f64_f64            methods/flow_accumulation.hpp:28 (FA_D4<double, double>); accum_inout holds the weights
+ * Peak device memory per cell (beyond the float engine's own scratch): see INTEGRATION.md. */
+RDB200_API int rdb200_fill_depressions_d8_f64(double *dem, int32_t width, int32_t height);
+RDB200_API int rdb200_fill_depressions_d4_f64(double *dem, int32_t width, int32_t height);
+RDB200_API int rdb200_pit_mask_d8_f64(const double *dem, uint8_t *mask, int32_t width, int32_t height, double nodata);
+RDB200_API int rdb200_pit_mask_d4_f64(const double *dem, uint8_t *mask, int32_t width, int32_t height, double nodata);
+RDB200_API int rdb200_has_depressions_d8_f64(const double *dem, int32_t width, int32_t height, int32_t *out);
+RDB200_API int rdb200_has_depressions_d4_f64(const double *dem, int32_t width, int32_t height, int32_t *out);
+RDB200_API int rdb200_resolve_flats_epsilon_f64(double *dem, int32_t width, int32_t height, double nodata);
+RDB200_API int rdb200_d8_flow_directions_f64(const double *dem, uint8_t *flowdirs, int32_t width, int32_t height,
+                                             double nodata);
+RDB200_API int rdb200_fa_d8_f64_f64(const double *dem, double *accum_inout, int32_t width, int32_t height, double nodata,
+                                    int32_t accum_is_ones);
+RDB200_API int rdb200_fa_d4_f64_f64(const double *dem, double *accum_inout, int32_t width, int32_t height, double nodata);
+/* DIAGNOSTIC, not part of the stable interface: the key encoding is an implementation detail of the entry points above
+ * and may change between versions (tests use these two to check it).  kappa itself: keys (width x height floats), *nodata_key = kappa(nodata) (the key of a cell equal to nodata; else the
+ * image of +-inf / +-DBL_MAX when nodata is one; else NaN), *ranked = 0 for the cast to float, 1 for dense ranks
+ * (__uint_as_float(0x00800000 + rank); +-inf, +-DBL_MAX and NaN keep the images +-inf, +-FLT_MAX and NaN).
+ * nodata_key and ranked may be null. */
+RDB200_API int rdb200_f64_order_keys(const double *dem, float *keys, int32_t width, int32_t height, double nodata,
+                                     float *nodata_key, int32_t *ranked);
+
 /* richdem::TA_slope_riserun / TA_slope_percentage / TA_slope_degrees / TA_slope_radians / TA_aspect / TA_curvature /
  * TA_planform_curvature / TA_profile_curvature(const Array2D<float>&, Array2D<float>&, float zscale)
  *   include/richdem/methods/terrain_attributes.hpp:370-538 over TerrainProcessor (:336-354) and the per-cell
@@ -256,6 +290,23 @@ RDB200_API int rdb200_dev_fa_d8_f32_f64(const float *d_dem, double *d_accum_inou
                              int32_t height, float nodata, int32_t accum_is_ones);
 RDB200_API int rdb200_dev_fa_tarboton_f32_f64(const float *d_dem, double *d_accum_inout, int32_t width,
                                    int32_t height, float nodata, int32_t accum_is_ones);
+/* the float64 entry points on device pointers (d_dem of pit_mask / has_depressions / d8 / fa is not modified) */
+RDB200_API int rdb200_dev_fill_depressions_d8_f64(double *d_dem, int32_t width, int32_t height);
+RDB200_API int rdb200_dev_fill_depressions_d4_f64(double *d_dem, int32_t width, int32_t height);
+RDB200_API int rdb200_dev_pit_mask_d8_f64(const double *d_dem, uint8_t *d_mask, int32_t width, int32_t height, double nodata);
+RDB200_API int rdb200_dev_pit_mask_d4_f64(const double *d_dem, uint8_t *d_mask, int32_t width, int32_t height, double nodata);
+RDB200_API int rdb200_dev_has_depressions_d8_f64(const double *d_dem, int32_t width, int32_t height, int32_t *out);
+RDB200_API int rdb200_dev_has_depressions_d4_f64(const double *d_dem, int32_t width, int32_t height, int32_t *out);
+RDB200_API int rdb200_dev_resolve_flats_epsilon_f64(double *d_dem, int32_t width, int32_t height, double nodata);
+RDB200_API int rdb200_dev_d8_flow_directions_f64(const double *d_dem, uint8_t *d_flowdirs, int32_t width, int32_t height,
+                                                 double nodata);
+RDB200_API int rdb200_dev_fa_d8_f64_f64(const double *d_dem, double *d_accum_inout, int32_t width, int32_t height,
+                                        double nodata, int32_t accum_is_ones);
+RDB200_API int rdb200_dev_fa_d4_f64_f64(const double *d_dem, double *d_accum_inout, int32_t width, int32_t height,
+                                        double nodata);
+/* diagnostic, as rdb200_f64_order_keys */
+RDB200_API int rdb200_dev_f64_order_keys(const double *d_dem, float *d_keys, int32_t width, int32_t height, double nodata,
+                                         float *nodata_key, int32_t *ranked);
 
 /* Seeded synthetic fractal DEM (value-noise fBm, float32, no NaN / NoData) generated in HBM;
  * benchmark input only (the reference's generate_perlin_terrain is single-octave/double:

@@ -349,6 +349,87 @@ RICHDEM_B200_TA(TA_profile_curvature, RDB200_TA_PROFILE_CURVATURE)
 #undef RICHDEM_B200_TA
 #endif
 
+#ifdef RICHDEM_B200_F64
+// float64 elevations (opt-in: `#define RICHDEM_B200_F64` before this include).  Without the macro Array2D<double> keeps
+// the reference's CPU templates.  Each specialisation below forwards to the rdb200_*_f64 entry point of the same
+// reference function; the results are the double templates' bit for bit, the fill's zero sign aside (DESIGN §0.1).
+// depressions/depressions.hpp:13-21 -> Zhou2016.hpp:125-191 (D8) / Barnes2014.hpp:230-304 (D4)
+template <>
+inline void FillDepressions<Topology::D8, double>(Array2D<double> &dem) {
+  richdem_b200::check(rdb200_fill_depressions_d8_f64(dem.data(), dem.width(), dem.height()));
+}
+template <>
+inline void FillDepressions<Topology::D4, double>(Array2D<double> &dem) {
+  richdem_b200::check(rdb200_fill_depressions_d4_f64(dem.data(), dem.width(), dem.height()));
+}
+template <>
+inline void PriorityFlood_Zhou2016<double>(Array2D<double> &dem) {
+  richdem_b200::check(rdb200_fill_depressions_d8_f64(dem.data(), dem.width(), dem.height()));
+}
+template <>
+inline void PriorityFlood_Barnes2014<Topology::D4, double>(Array2D<double> &dem) {
+  richdem_b200::check(rdb200_fill_depressions_d4_f64(dem.data(), dem.width(), dem.height()));
+}
+// depressions/Barnes2014.hpp:593-676 and :43-104
+template <>
+inline void pit_mask<Topology::D8, double>(const Array2D<double> &elevations, Array2D<uint8_t> &mask) {
+  mask.resize(elevations.width(), elevations.height());
+  mask.setNoData(3);
+  richdem_b200::check(rdb200_pit_mask_d8_f64(elevations.data(), mask.data(), elevations.width(), elevations.height(),
+                                             elevations.noData()));
+}
+template <>
+inline void pit_mask<Topology::D4, double>(const Array2D<double> &elevations, Array2D<uint8_t> &mask) {
+  mask.resize(elevations.width(), elevations.height());
+  mask.setNoData(3);
+  richdem_b200::check(rdb200_pit_mask_d4_f64(elevations.data(), mask.data(), elevations.width(), elevations.height(),
+                                             elevations.noData()));
+}
+template <>
+inline bool HasDepressions<Topology::D8, double>(const Array2D<double> &elevations) {
+  int32_t any = 0;
+  richdem_b200::check(rdb200_has_depressions_d8_f64(elevations.data(), elevations.width(), elevations.height(), &any));
+  return any != 0;
+}
+template <>
+inline bool HasDepressions<Topology::D4, double>(const Array2D<double> &elevations) {
+  int32_t any = 0;
+  richdem_b200::check(rdb200_has_depressions_d4_f64(elevations.data(), elevations.width(), elevations.height(), &any));
+  return any != 0;
+}
+// flats/flats.hpp:21-28
+template <>
+inline void ResolveFlatsEpsilon<double>(Array2D<double> &elevations) {
+  richdem_b200::check(rdb200_resolve_flats_epsilon_f64(elevations.data(), elevations.width(), elevations.height(),
+                                                       elevations.noData()));
+}
+// flowmet/d8_flowdirs.hpp:96-123
+template <>
+inline void d8_flow_directions<double, uint8_t>(const Array2D<double> &elevations, Array2D<uint8_t> &flowdirs) {
+  flowdirs.resize(elevations);
+  flowdirs.setNoData(FLOWDIR_NO_DATA);
+  richdem_b200::check(rdb200_d8_flow_directions_f64(elevations.data(), flowdirs.data(), elevations.width(),
+                                                    elevations.height(), elevations.noData()));
+}
+// methods/flow_accumulation.hpp:27,28; accum holds the weights, as for float
+template <>
+inline void FA_D8<double, double>(const Array2D<double> &elevations, Array2D<double> &accum) {
+  accum.setNoData(ACCUM_NO_DATA);
+  if (accum.width() != elevations.width() || accum.height() != elevations.height())
+    throw std::runtime_error("Accumulation array must have same dimensions as proportions array!");
+  richdem_b200::check(rdb200_fa_d8_f64_f64(elevations.data(), accum.data(), elevations.width(), elevations.height(),
+                                           elevations.noData(), 0));
+}
+template <>
+inline void FA_D4<double, double>(const Array2D<double> &elevations, Array2D<double> &accum) {
+  accum.setNoData(ACCUM_NO_DATA);
+  if (accum.width() != elevations.width() || accum.height() != elevations.height())
+    throw std::runtime_error("Accumulation array must have same dimensions as proportions array!");
+  richdem_b200::check(rdb200_fa_d4_f64_f64(elevations.data(), accum.data(), elevations.width(), elevations.height(),
+                                           elevations.noData()));
+}
+#endif  // RICHDEM_B200_F64
+
 }  // namespace richdem
 
 #endif

@@ -106,7 +106,8 @@ def _dem_f32(dem: rdarray, what: str) -> np.ndarray:
     if dem.dtype != np.float32:
         raise Exception(
             f"{what}: the H100 path is built for float32 elevations (got '{dem.dtype}'); "
-            "convert with dem.astype('float32') -- there is no CPU fallback for other dtypes.")
+            "convert with dem.astype('float32') -- there is no CPU fallback for other dtypes "
+            "(float64 rasters: richdem_b200.f64 computes the float64 answer).")
     if not dem.flags["C_CONTIGUOUS"]:
         raise Exception(f"{what}: the raster must be C-contiguous")
     return dem

@@ -35,7 +35,7 @@ class Stats(C.Structure):
 
 
 # every symbol include/richdem_b200.h declares: name -> argtypes (restype is int unless noted)
-_i32, _f32, _vp = C.c_int32, C.c_float, C.c_void_p
+_i32, _f32, _f64, _vp = C.c_int32, C.c_float, C.c_double, C.c_void_p
 SIGNATURES = {
     "rdb200_init": [C.c_int],
     "rdb200_set_stream": [C.c_void_p],
@@ -88,6 +88,28 @@ SIGNATURES = {
     "rdb200_dev_flow_accumulation_props_f64": [_vp, _vp, _i32, _i32],
     "rdb200_dev_fa_d8_f32_f64": [_vp, _vp, _i32, _i32, _f32, _i32],
     "rdb200_dev_fa_tarboton_f32_f64": [_vp, _vp, _i32, _i32, _f32, _i32],
+    "rdb200_fill_depressions_d8_f64": [_vp, _i32, _i32],
+    "rdb200_fill_depressions_d4_f64": [_vp, _i32, _i32],
+    "rdb200_pit_mask_d8_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_pit_mask_d4_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_has_depressions_d8_f64": [_vp, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_has_depressions_d4_f64": [_vp, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_resolve_flats_epsilon_f64": [_vp, _i32, _i32, _f64],
+    "rdb200_d8_flow_directions_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_fa_d8_f64_f64": [_vp, _vp, _i32, _i32, _f64, _i32],
+    "rdb200_fa_d4_f64_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_f64_order_keys": [_vp, _vp, _i32, _i32, _f64, C.POINTER(_f32), C.POINTER(_i32)],
+    "rdb200_dev_fill_depressions_d8_f64": [_vp, _i32, _i32],
+    "rdb200_dev_fill_depressions_d4_f64": [_vp, _i32, _i32],
+    "rdb200_dev_pit_mask_d8_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_dev_pit_mask_d4_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_dev_has_depressions_d8_f64": [_vp, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_dev_has_depressions_d4_f64": [_vp, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_dev_resolve_flats_epsilon_f64": [_vp, _i32, _i32, _f64],
+    "rdb200_dev_d8_flow_directions_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_dev_fa_d8_f64_f64": [_vp, _vp, _i32, _i32, _f64, _i32],
+    "rdb200_dev_fa_d4_f64_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_dev_f64_order_keys": [_vp, _vp, _i32, _i32, _f64, C.POINTER(_f32), C.POINTER(_i32)],
     "rdb200_dev_generate_fbm_f32": [_vp, _i32, _i32, _i32, C.c_uint32, _i32, _f32],
     "rdb200_nccl_unique_id": [_vp],
     "rdb200_comm_create_nccl": [C.POINTER(_vp), _i32, _i32, _vp],

@@ -8,7 +8,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "librichdem_b200.so")
-SOURCES = ["capi.cu", "comm.cu", "fill.cu", "flats.cu", "flowdirs.cu", "accum.cu", "terrain.cu", "attributes.cu", "depressions.cu"]
+SOURCES = ["capi.cu", "comm.cu", "fill.cu", "flats.cu", "flowdirs.cu", "accum.cu", "terrain.cu", "attributes.cu", "depressions.cu",
+           "f64.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
     *GENCODE,

@@ -564,6 +564,167 @@ int rdb200_fa_tarboton_f32_f64(const float *dem, double *accum, int32_t w, int32
   return fa_host(dem, accum, w, h, nodata, ones, true);
 }
 
+// ---- float64 rasters (f64.cu): the float engines on kappa(Z), kappa an order-preserving map to float keys ------------
+
+// reference depressions/depressions.hpp:13-21 -> Zhou2016.hpp:125-191 (D8) / Barnes2014.hpp:230-304 (D4), T = double
+int rdb200_fill_depressions_d8_f64(double *dem, int32_t w, int32_t h) {
+  CAPI_TRY
+  if (!dem) fail("fill_depressions: null dem");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n);
+  h2d(d.p, dem, n);
+  fill_depressions_f64_dev(d.p, w, h, false);
+  d2h(dem, d.p, n);
+  cs.done();
+  CAPI_END
+}
+int rdb200_fill_depressions_d4_f64(double *dem, int32_t w, int32_t h) {
+  CAPI_TRY
+  if (!dem) fail("fill_depressions: null dem");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n);
+  h2d(d.p, dem, n);
+  fill_depressions_f64_dev(d.p, w, h, true);
+  d2h(dem, d.p, n);
+  cs.done();
+  CAPI_END
+}
+
+// reference depressions/Barnes2014.hpp:593-676 (pit_mask<topo>, T = double)
+static int pit_mask_f64_host(const double *dem, uint8_t *mask, int32_t w, int32_t h, double nodata, bool topo4) {
+  CAPI_TRY
+  if (!dem || !mask) fail("pit_mask: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n);
+  DevBuf<uint8_t> m(n);
+  h2d(d.p, dem, n);
+  pit_mask_f64_dev(d.p, m.p, w, h, nodata, topo4);
+  d2h(mask, m.p, n);
+  cs.done();
+  CAPI_END
+}
+int rdb200_pit_mask_d8_f64(const double *dem, uint8_t *mask, int32_t w, int32_t h, double nodata) {
+  return pit_mask_f64_host(dem, mask, w, h, nodata, false);
+}
+int rdb200_pit_mask_d4_f64(const double *dem, uint8_t *mask, int32_t w, int32_t h, double nodata) {
+  return pit_mask_f64_host(dem, mask, w, h, nodata, true);
+}
+
+// reference depressions/Barnes2014.hpp:43-104 (HasDepressions<topo>, T = double)
+static int has_depressions_f64_host(const double *dem, int32_t w, int32_t h, int32_t *out, bool topo4) {
+  CAPI_TRY
+  if (!dem || !out) fail("has_depressions: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n);
+  h2d(d.p, dem, n);
+  const bool any = has_depressions_f64_dev(d.p, w, h, topo4);
+  cs.done();
+  *out = any ? 1 : 0;
+  CAPI_END
+}
+int rdb200_has_depressions_d8_f64(const double *dem, int32_t w, int32_t h, int32_t *out) {
+  return has_depressions_f64_host(dem, w, h, out, false);
+}
+int rdb200_has_depressions_d4_f64(const double *dem, int32_t w, int32_t h, int32_t *out) {
+  return has_depressions_f64_host(dem, w, h, out, true);
+}
+
+// reference flats/flats.hpp:21-28 -> flats/Barnes2014.hpp:398-467 (GetFlatMask) + :496-550 (apply), T = double
+int rdb200_resolve_flats_epsilon_f64(double *dem, int32_t w, int32_t h, double nodata) {
+  CAPI_TRY
+  if (!dem) fail("resolve_flats: null dem");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n);
+  h2d(d.p, dem, n);
+  resolve_flats_f64_dev(d.p, w, h, nodata);
+  d2h(dem, d.p, n);
+  cs.done();
+  CAPI_END
+}
+
+// reference flowmet/d8_flowdirs.hpp:32-123 (d8_flow_directions<double, uint8_t>)
+int rdb200_d8_flow_directions_f64(const double *dem, uint8_t *dirs, int32_t w, int32_t h, double nodata) {
+  CAPI_TRY
+  if (!dem || !dirs) fail("d8_flow_directions: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n);
+  DevBuf<uint8_t> o(n);
+  h2d(d.p, dem, n);
+  d8_flow_directions_f64_dev(d.p, o.p, w, h, nodata);
+  d2h(dirs, o.p, n);
+  cs.done();
+  CAPI_END
+}
+
+// reference methods/flow_accumulation.hpp:27 (FA_D8<double, double>: OCallaghan1984.hpp:13-91 + flow_accumulation_generic.hpp:33-100)
+int rdb200_fa_d8_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata, int32_t ones) {
+  CAPI_TRY
+  if (!dem || !accum) fail("flow accumulation: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n), a(n);
+  h2d(d.p, dem, n);
+  if (!ones) h2d(a.p, accum, n);
+  fa_d8_f64_dev(d.p, a.p, w, h, nodata, ones != 0);
+  d2h(accum, a.p, n);
+  cs.done();
+  CAPI_END
+}
+
+// reference methods/flow_accumulation.hpp:28 (FA_D4<double, double>: OCallaghan1984.hpp:89-91 + the generic accumulation)
+static void fa_d4_f64_dev(const double *d_dem, double *d_accum, int w, int h, double nodata) {
+  DevBuf<float> key((size_t)w * h);
+  const float nd = f64_keys_dev(d_dem, key.p, (size_t)w * h, nodata, nullptr, nullptr);
+  fa_via_props_dev(2, key.p, d_accum, w, h, nd, 0);
+}
+int rdb200_fa_d4_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata) {
+  CAPI_TRY
+  if (!dem || !accum) fail("flow accumulation: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n), a(n);
+  h2d(d.p, dem, n);
+  h2d(a.p, accum, n);
+  fa_d4_f64_dev(d.p, a.p, w, h, nodata);
+  d2h(accum, a.p, n);
+  cs.done();
+  CAPI_END
+}
+
+// kappa itself: the float keys the entry points above run the float engines on, kappa(nodata) and which case ran
+int rdb200_f64_order_keys(const double *dem, float *keys, int32_t w, int32_t h, double nodata, float *nodata_key,
+                          int32_t *ranked) {
+  CAPI_TRY
+  if (!dem || !keys) fail("f64_order_keys: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n);
+  DevBuf<float> k(n);
+  h2d(d.p, dem, n);
+  int r = 0;
+  const float nd = f64_keys_dev(d.p, k.p, n, nodata, nullptr, &r);
+  d2h(keys, k.p, n);
+  cs.done();
+  if (nodata_key) *nodata_key = nd;
+  if (ranked) *ranked = r;
+  CAPI_END
+}
+
 // ---- device entry points ------------------------------------------------------------------------
 
 #define DEV_ENTRY(cells, body) \
@@ -652,6 +813,70 @@ int rdb200_dev_terrain_attribute_f32(int32_t attribute, const float *d_dem, floa
   DEV_ENTRY((int64_t)w * h, (check_dims(w, h), terrain_attribute_dev(attribute, d_dem, d_out, w, h, nodata_in, nodata_out, zscale,
                                                                     cell_x, cell_y)))
 }
+// float64 twins of the host entry points above, on device pointers (the reference lines are cited there)
+int rdb200_dev_fill_depressions_d8_f64(double *d_dem, int32_t w, int32_t h) {
+  DEV_ENTRY((int64_t)w * h, (check_dims(w, h), fill_depressions_f64_dev(d_dem, w, h, false)))
+}
+int rdb200_dev_fill_depressions_d4_f64(double *d_dem, int32_t w, int32_t h) {
+  DEV_ENTRY((int64_t)w * h, (check_dims(w, h), fill_depressions_f64_dev(d_dem, w, h, true)))
+}
+static int dev_pit_mask_f64(const double *d_dem, uint8_t *d_mask, int32_t w, int32_t h, double nodata, bool topo4) {
+  CAPI_TRY
+  if (!d_dem || !d_mask) fail("pit_mask: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  pit_mask_f64_dev(d_dem, d_mask, w, h, nodata, topo4);
+  cs.done();
+  CAPI_END
+}
+int rdb200_dev_pit_mask_d8_f64(const double *d_dem, uint8_t *d_mask, int32_t w, int32_t h, double nodata) {
+  return dev_pit_mask_f64(d_dem, d_mask, w, h, nodata, false);
+}
+int rdb200_dev_pit_mask_d4_f64(const double *d_dem, uint8_t *d_mask, int32_t w, int32_t h, double nodata) {
+  return dev_pit_mask_f64(d_dem, d_mask, w, h, nodata, true);
+}
+static int dev_has_depressions_f64(const double *d_dem, int32_t w, int32_t h, int32_t *out, bool topo4) {
+  CAPI_TRY
+  if (!d_dem || !out) fail("has_depressions: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const bool any = has_depressions_f64_dev(d_dem, w, h, topo4);
+  cs.done();
+  *out = any ? 1 : 0;
+  CAPI_END
+}
+int rdb200_dev_has_depressions_d8_f64(const double *d_dem, int32_t w, int32_t h, int32_t *out) {
+  return dev_has_depressions_f64(d_dem, w, h, out, false);
+}
+int rdb200_dev_has_depressions_d4_f64(const double *d_dem, int32_t w, int32_t h, int32_t *out) {
+  return dev_has_depressions_f64(d_dem, w, h, out, true);
+}
+int rdb200_dev_resolve_flats_epsilon_f64(double *d_dem, int32_t w, int32_t h, double nodata) {
+  DEV_ENTRY((int64_t)w * h, (check_dims(w, h), resolve_flats_f64_dev(d_dem, w, h, nodata)))
+}
+int rdb200_dev_d8_flow_directions_f64(const double *d_dem, uint8_t *d_dirs, int32_t w, int32_t h, double nodata) {
+  DEV_ENTRY((int64_t)w * h, (check_dims(w, h), d8_flow_directions_f64_dev(d_dem, d_dirs, w, h, nodata)))
+}
+int rdb200_dev_fa_d8_f64_f64(const double *d_dem, double *d_accum, int32_t w, int32_t h, double nodata, int32_t ones) {
+  DEV_ENTRY((int64_t)w * h, (check_dims(w, h), fa_d8_f64_dev(d_dem, d_accum, w, h, nodata, ones != 0)))
+}
+int rdb200_dev_fa_d4_f64_f64(const double *d_dem, double *d_accum, int32_t w, int32_t h, double nodata) {
+  DEV_ENTRY((int64_t)w * h, (check_dims(w, h), fa_d4_f64_dev(d_dem, d_accum, w, h, nodata)))
+}
+int rdb200_dev_f64_order_keys(const double *d_dem, float *d_keys, int32_t w, int32_t h, double nodata, float *nodata_key,
+                              int32_t *ranked) {
+  CAPI_TRY
+  if (!d_dem || !d_keys) fail("f64_order_keys: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  int r = 0;
+  const float nd = f64_keys_dev(d_dem, d_keys, (size_t)w * h, nodata, nullptr, &r);
+  cs.done();
+  if (nodata_key) *nodata_key = nd;
+  if (ranked) *ranked = r;
+  CAPI_END
+}
+
 int rdb200_dev_generate_fbm_f32(float *d_dem, int32_t w, int32_t h, int32_t y0, uint32_t seed, int32_t octaves,
                                 float quantum) {
   DEV_ENTRY((int64_t)w * h, (check_dims(w, h), generate_fbm_dev(d_dem, w, h, y0, seed, octaves, quantum)))

@@ -211,5 +211,19 @@ void mgpu_pit_mask_band(const rdb200_comm *comm, const float *d_band, uint8_t *d
                         int gb, int row0, int H, bool topo4);
 bool mgpu_has_depressions_band(const rdb200_comm *comm, const float *d_band, int w, int hloc, int gt, int gb, int row0, int H,
                                bool topo4);
+// pit_mask's compare pass (mask may be null) and the strict-pit stencil, OR-ed into the device flags
+void pit_mask_compare_dev(const float *d_z, const float *d_l, uint8_t *d_mask, size_t n, float nodata, int *d_any);
+void strict_pit_f64_dev(const double *d_z, int w, int h, bool topo4, int *d_flag);
+void d8_flow_directions_f64_dev(const double *d_dem, uint8_t *d_dirs, int w, int h, double nodata);
+
+// ---- float64 rasters through order-preserving float keys (f64.cu) ---------------------------
+// kappa(Z) of n doubles into d_key; returns kappa(nodata).  *ranked (may be null): 0 when kappa is the cast to float,
+// 1 when it is the dense rank.  With table, case 2 allocates the kappa^-1 table of sorted distinct values (n doubles).
+float f64_keys_dev(const double *d_z, float *d_key, size_t n, double nodata, DevBuf<double> *table, int *ranked);
+void fill_depressions_f64_dev(double *d_z, int w, int h, bool topo4);
+void pit_mask_f64_dev(const double *d_z, uint8_t *d_mask, int w, int h, double nodata, bool topo4);
+bool has_depressions_f64_dev(const double *d_z, int w, int h, bool topo4);
+void resolve_flats_f64_dev(double *d_z, int w, int h, double nodata);
+void fa_d8_f64_dev(const double *d_z, double *d_accum, int w, int h, double nodata, bool ones);
 
 }  // namespace rdb

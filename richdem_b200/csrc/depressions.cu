@@ -68,8 +68,9 @@ __global__ void __launch_bounds__(256) pit_mask_kernel(const float *__restrict__
 //
 // One thread per column walks PIT_ROWS rows of a block's strip with a three-row window in registers; the left and right
 // neighbours are the adjacent threads' loads (L1 hits).  Blocks stop early once another block has found a pit.
-template <bool TOPO4>
-__global__ void __launch_bounds__(256) strict_pit_kernel(const float *__restrict__ Z, int W, int H, int *flag) {
+// T is float, or double for the float64 entry points (f64.cu), which compare their doubles directly here.
+template <bool TOPO4, class T>
+__global__ void __launch_bounds__(256) strict_pit_kernel(const T *__restrict__ Z, int W, int H, int *flag) {
   const int x = 1 + blockIdx.x * blockDim.x + threadIdx.x;
   const int strips = (H - 2 + PIT_ROWS - 1) / PIT_ROWS;
   int found = 0;
@@ -77,13 +78,13 @@ __global__ void __launch_bounds__(256) strict_pit_kernel(const float *__restrict
     for (int s = blockIdx.y; s < strips && !found; s += gridDim.y) {
       if (*(volatile int *)flag) break;
       const int y0 = 1 + s * PIT_ROWS, y1 = y0 + PIT_ROWS < H - 1 ? y0 + PIT_ROWS : H - 1;
-      const float *r = Z + (size_t)(y0 - 1) * W + x;
-      float ul = r[-1], uc = r[0], ur = r[1];
+      const T *r = Z + (size_t)(y0 - 1) * W + x;
+      T ul = r[-1], uc = r[0], ur = r[1];
       r += W;
-      float cl = r[-1], cc = r[0], cr = r[1];
+      T cl = r[-1], cc = r[0], cr = r[1];
       for (int y = y0; y < y1; y++) {
         r += W;
-        const float dl = r[-1], dc = r[0], dr = r[1];
+        const T dl = r[-1], dc = r[0], dr = r[1];
         bool pit = cc < cl && cc < cr && cc < uc && cc < dc;
         if (!TOPO4) pit = pit && cc < ul && cc < ur && cc < dl && cc < dr;
         found |= pit;
@@ -119,15 +120,20 @@ void pit_mask_compare_dev(const float *d_z, const float *d_l, uint8_t *d_mask, s
 }
 
 // strict-pit pass over a w x h raster whose first and last rows and columns are not tested; OR-ed into *d_flag
-void strict_pit_dev(const float *d_z, int w, int h, bool topo4, int *d_flag) {
+template <class T>
+static void strict_pit_launch(const T *d_z, int w, int h, bool topo4, int *d_flag) {
   Ctx &c = ctx();
   if (w < 3 || h < 3) return;
   const int strips = (h - 2 + PIT_ROWS - 1) / PIT_ROWS;
   dim3 blk(256), grd((unsigned)((w - 2 + 255) / 256), (unsigned)(strips < 65535 ? strips : 65535));
-  if (topo4) strict_pit_kernel<true><<<grd, blk, 0, c.stream>>>(d_z, w, h, d_flag);
-  else strict_pit_kernel<false><<<grd, blk, 0, c.stream>>>(d_z, w, h, d_flag);
+  if (topo4) strict_pit_kernel<true, T><<<grd, blk, 0, c.stream>>>(d_z, w, h, d_flag);
+  else strict_pit_kernel<false, T><<<grd, blk, 0, c.stream>>>(d_z, w, h, d_flag);
   RDB_CK(cudaGetLastError());
   count_launch();
+}
+void strict_pit_dev(const float *d_z, int w, int h, bool topo4, int *d_flag) { strict_pit_launch(d_z, w, h, topo4, d_flag); }
+void strict_pit_f64_dev(const double *d_z, int w, int h, bool topo4, int *d_flag) {
+  strict_pit_launch(d_z, w, h, topo4, d_flag);
 }
 
 // L = the fill of d_dem, in a scratch copy (the fill relaxes its water surface in the raster it is handed)

@@ -1,0 +1,519 @@
+// float64 rasters through order-preserving float keys (DESIGN §0 "float64 elevations").
+//
+// FillDepressions<D8/D4>, pit_mask, HasDepressions, ResolveFlatsEpsilon, d8_flow_directions, FA_D8 and FA_D4 use an
+// elevation in only three ways: they compare it with other elevations, with the raster's NoData value and with
+// numeric_limits<T>::max(); the fill copies one cell's value into another; and the flats' last step applies
+// nextafter(z, +inf) k times.  So for a map kappa from doubles to floats that is strictly increasing on the raster's
+// values, sends DBL_MAX, -DBL_MAX, +-inf and NaN to FLT_MAX, -FLT_MAX, +-inf and NaN, and gives -0.0 and +0.0 keys that
+// compare equal, the float engine on kappa(Z) takes the control flow the double template takes on Z, and every value it
+// copies is kappa of the value the double run copies.  This file builds kappa(Z) (the only new hot path), maps a filled
+// key raster back to doubles, and applies the flats' increment mask as double ulps.  The float engines run unchanged.
+//
+// kappa, chosen by looking at the input:
+//   case 1  every value is NaN, +-inf or a float-exact double with |z| < FLT_MAX (a widened float raster):
+//           kappa(z) = (float)z, one pass.  A cell at +-FLT_MAX goes to case 2: its image would collide with DBL_MAX's.
+//   case 2  dense ranks: sort (order key, cell) pairs by an LSD radix sort over the 8-bit digits that are not the same
+//           for every key, rank the runs of equal values (+-0 together, every NaN apart), and give rank r the key
+//           __uint_as_float(0x00800000 + r): positive normals, strictly inside (-FLT_MAX, FLT_MAX) because a raster
+//           holds fewer than 2^31 - 2^25 cells.  The sorted distinct doubles are the inverse table.
+// kappa(nodata) is the key of a cell equal to nodata; without one, the constant's image when nodata is one, else NaN
+// (which equals nothing, as nodata then does).
+//
+// Everything here uses plain loads, shared-memory atomics, barriers and full-mask warp collectives (no TMA, no PTX), so
+// the test suite's CPU model of the kernels runs it as it runs the float engines.
+#include "common.cuh"
+
+#include <cfloat>
+
+namespace rdb {
+
+namespace {
+
+constexpr int SORT_THREADS = 256;  // every kernel below assumes 256 threads (8 warps) per block
+constexpr int SORT_ITEMS = 16;
+constexpr int SORT_TILE = SORT_THREADS * SORT_ITEMS;  // cells per tile of a sort pass, entries per chunk of a scan
+constexpr uint32_t RANK_BASE = 0x00800000u;           // FLT_MIN: the key of rank 0
+constexpr unsigned FULL = 0xffffffffu;
+constexpr uint32_t NO_KEY = 0xffffffffu;  // "no cell equals nodata" (a NaN pattern: never the key of a cell equal to it)
+
+// monotone uint64 image of a double (negative values reversed below the positive ones); -0.0 sits just below +0.0
+__device__ __forceinline__ uint64_t order_key(double v) {
+  const uint64_t b = (uint64_t)__double_as_longlong(v);
+  return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+__device__ __forceinline__ double order_value(uint64_t k) {
+  return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+
+__device__ __forceinline__ float rank_key(double v, uint32_t r) {
+  if (v != v) return __uint_as_float(0x7fc00000u);
+  if (v == (double)INFINITY) return INFINITY;
+  if (v == -(double)INFINITY) return -INFINITY;
+  if (v == DBL_MAX) return FLT_MAX;
+  if (v == -DBL_MAX) return -FLT_MAX;
+  return __uint_as_float(RANK_BASE + r);
+}
+
+// kappa^-1 of a key the float engine produced (table: case 2's sorted distinct doubles, null in case 1)
+__device__ __forceinline__ double key_value(float k, const double *__restrict__ table) {
+  if (k != k) return __longlong_as_double(0x7ff8000000000000ll);
+  if (k == INFINITY) return (double)INFINITY;
+  if (k == -INFINITY) return -(double)INFINITY;
+  if (!table) return (double)k;
+  if (k == FLT_MAX) return DBL_MAX;
+  if (k == -FLT_MAX) return -DBL_MAX;
+  return table[__float_as_uint(k) - RANK_BASE];
+}
+
+// case 1, speculatively: key = (float)z; *inexact = 1 if some value is none of NaN, +-inf, a float-exact |z| < FLT_MAX.
+// *nd_key receives the key of some cell equal to nodata.
+__global__ void __launch_bounds__(256) f64_cast_kernel(const double *__restrict__ z, float *__restrict__ key, size_t n,
+                                                       double nodata, int *inexact, uint32_t *nd_key) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  int bad = 0, found = 0;
+  uint32_t nd_bits = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const double v = z[i];
+    const float f = (float)v;
+    const bool special = v != v || v == (double)INFINITY || v == -(double)INFINITY;
+    if (!special && !((double)f == v && fabs(v) < (double)FLT_MAX)) bad = 1;
+    if (v == nodata) {
+      found = 1;
+      nd_bits = __float_as_uint(f);
+    }
+    key[i] = f;
+  }
+  if (found) *nd_key = nd_bits;  // cells equal to nodata share a key (up to the sign of a zero): any writer will do
+  if (__syncthreads_or(bad) && threadIdx.x == 0) *inexact = 1;
+}
+
+// the (order key, cell) pair at position i: from the previous pass's output, or straight from Z before the first pass
+__device__ __forceinline__ void load_pair(size_t i, const uint64_t *__restrict__ ks, const uint32_t *__restrict__ is,
+                                          const double *__restrict__ z, uint64_t &k, uint32_t &idx) {
+  if (z) {
+    k = order_key(z[i]);
+    idx = (uint32_t)i;
+  } else {
+    k = ks[i];
+    idx = is[i];
+  }
+}
+
+// all eight digit histograms in one pass: hist[d * 256 + b] counts the keys whose digit d (bits 8d..8d+7) is b
+__global__ void __launch_bounds__(256) digit_hist_kernel(const double *__restrict__ z, size_t n, uint32_t *hist) {
+  __shared__ uint32_t s[8 * 256];
+  for (int k = threadIdx.x; k < 8 * 256; k += blockDim.x) s[k] = 0;
+  __syncthreads();
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const uint64_t k = order_key(z[i]);
+#pragma unroll
+    for (int d = 0; d < 8; d++) atomicAdd(&s[d * 256 + (int)((k >> (8 * d)) & 255u)], 1u);
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < 8 * 256; k += blockDim.x)
+    if (s[k]) atomicAdd(&hist[k], s[k]);
+}
+
+// exclusive scan of one value per thread over the block (256 threads); total = the block's sum.  ws: 8 shared words.
+__device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t *ws, uint32_t &total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  uint32_t x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t y = __shfl_up_sync(FULL, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) ws[wid] = x;
+  __syncthreads();
+  uint32_t before = 0;
+  total = 0;
+#pragma unroll
+  for (int k = 0; k < 8; k++) {
+    const uint32_t s = ws[k];
+    if (k < wid) before += s;
+    total += s;
+  }
+  __syncthreads();  // ws is reused by the next call
+  return before + x - v;
+}
+
+// per-tile digit counts of one sort pass, digit-major: counts[b * tiles + tile]
+__global__ void __launch_bounds__(256) tile_count_kernel(const uint64_t *__restrict__ ks, const double *__restrict__ z, size_t n,
+                                                         int shift, uint32_t *__restrict__ counts, uint32_t tiles) {
+  __shared__ uint32_t s[256];
+  s[threadIdx.x] = 0;
+  __syncthreads();
+  const size_t base = (size_t)blockIdx.x * SORT_TILE;
+  for (int r = 0; r < SORT_ITEMS; r++) {
+    const size_t i = base + (size_t)r * SORT_THREADS + threadIdx.x;
+    if (i < n) {
+      const uint64_t k = z ? order_key(z[i]) : ks[i];
+      atomicAdd(&s[(int)((k >> shift) & 255u)], 1u);
+    }
+  }
+  __syncthreads();
+  counts[(size_t)threadIdx.x * tiles + blockIdx.x] = s[threadIdx.x];
+}
+
+// stable scatter of one sort pass.  offsets[b * tiles + tile] is where the tile's first digit-b key goes.  The tile is
+// read in rounds of 256 consecutive cells; inside a round a key's place is the count of earlier same-digit keys of its
+// tile: earlier rounds (s_base), earlier warps (prefix of s_wcnt) and lower lanes (a peer mask from 8 ballots).
+__global__ void __launch_bounds__(256) tile_scatter_kernel(const uint64_t *__restrict__ ks, const uint32_t *__restrict__ is,
+                                                           const double *__restrict__ z, uint64_t *__restrict__ ko,
+                                                           uint32_t *__restrict__ io, size_t n, int shift,
+                                                           const uint32_t *__restrict__ offsets, uint32_t tiles) {
+  __shared__ uint32_t s_base[256];
+  __shared__ uint32_t s_wcnt[8][256];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  s_base[threadIdx.x] = offsets[(size_t)threadIdx.x * tiles + blockIdx.x];
+  const size_t base = (size_t)blockIdx.x * SORT_TILE;
+  for (int r = 0; r < SORT_ITEMS; r++) {
+#pragma unroll
+    for (int w = 0; w < 8; w++) s_wcnt[w][threadIdx.x] = 0;
+    __syncthreads();
+    const size_t i = base + (size_t)r * SORT_THREADS + threadIdx.x;
+    const bool valid = i < n;
+    uint64_t k = 0;
+    uint32_t idx = 0;
+    if (valid) load_pair(i, ks, is, z, k, idx);
+    const uint32_t d = (uint32_t)(k >> shift) & 255u;
+    uint32_t peers = __ballot_sync(FULL, valid);
+#pragma unroll
+    for (int b = 0; b < 8; b++) {
+      const uint32_t bit = (d >> b) & 1u;
+      const uint32_t bal = __ballot_sync(FULL, (int)bit);
+      peers &= bit ? bal : ~bal;
+    }
+    const int below = __popc(peers & ((1u << lane) - 1u));
+    if (valid && below == 0) s_wcnt[wid][d] = (uint32_t)__popc(peers);
+    __syncthreads();
+    {  // thread b: prefix of digit b over the warps, starting at the tile's running position
+      uint32_t run = s_base[threadIdx.x];
+#pragma unroll
+      for (int w = 0; w < 8; w++) {
+        const uint32_t c = s_wcnt[w][threadIdx.x];
+        s_wcnt[w][threadIdx.x] = run;
+        run += c;
+      }
+      s_base[threadIdx.x] = run;
+    }
+    __syncthreads();
+    if (valid) {
+      const uint32_t pos = s_wcnt[wid][d] + (uint32_t)below;
+      ko[pos] = k;
+      io[pos] = idx;
+    }
+    __syncthreads();  // s_wcnt is cleared for the next round
+  }
+}
+
+// entry sources of the chunk scans: a uint32 array, or the run heads of the sorted keys
+struct ArraySrc {
+  const uint32_t *a;
+  __device__ __forceinline__ uint32_t operator()(size_t i) const { return a[i]; }
+};
+struct HeadSrc {  // 1 where a run of equal values starts (compared as doubles: +-0 share a run, each NaN is its own)
+  const uint64_t *ks;
+  const double *z;
+  __device__ __forceinline__ uint32_t operator()(size_t i) const {
+    if (i == 0) return 1;
+    const double a = z ? z[i - 1] : order_value(ks[i - 1]);
+    const double b = z ? z[i] : order_value(ks[i]);
+    return !(a == b);
+  }
+};
+
+template <class Src>
+__global__ void __launch_bounds__(256) chunk_sum_kernel(Src src, size_t m, uint32_t *__restrict__ sums) {
+  __shared__ uint32_t ws[8];
+  const size_t base = (size_t)blockIdx.x * SORT_TILE;
+  uint32_t acc = 0;
+  for (int r = 0; r < SORT_ITEMS; r++) {
+    const size_t i = base + (size_t)r * SORT_THREADS + threadIdx.x;
+    if (i < m) acc += src(i);
+  }
+  uint32_t total;
+  block_exclusive_scan(acc, ws, total);
+  if (threadIdx.x == 0) sums[blockIdx.x] = total;
+}
+
+// exclusive scan of the chunk sums, one block: 16 consecutive entries per thread and a carry across 4096-entry steps
+__global__ void __launch_bounds__(256) sums_scan_kernel(uint32_t *sums, size_t nb) {
+  __shared__ uint32_t ws[8];
+  uint32_t carry = 0;
+  for (size_t c = 0; c < nb; c += SORT_TILE) {
+    const size_t b0 = c + (size_t)threadIdx.x * SORT_ITEMS;
+    uint32_t v[SORT_ITEMS], acc = 0;
+#pragma unroll
+    for (int j = 0; j < SORT_ITEMS; j++) {
+      v[j] = b0 + j < nb ? sums[b0 + j] : 0u;
+      acc += v[j];
+    }
+    uint32_t total;
+    uint32_t run = carry + block_exclusive_scan(acc, ws, total);
+#pragma unroll
+    for (int j = 0; j < SORT_ITEMS; j++) {
+      if (b0 + j < nb) sums[b0 + j] = run;
+      run += v[j];
+    }
+    carry += total;
+  }
+}
+
+// a[i] = exclusive prefix sum (chunk offsets from sums_scan_kernel)
+__global__ void __launch_bounds__(256) scan_apply_kernel(uint32_t *a, size_t m, const uint32_t *__restrict__ sums) {
+  __shared__ uint32_t ws[8];
+  const size_t base = (size_t)blockIdx.x * SORT_TILE;
+  uint32_t carry = sums[blockIdx.x];
+  for (int r = 0; r < SORT_ITEMS; r++) {
+    const size_t i = base + (size_t)r * SORT_THREADS + threadIdx.x;
+    const uint32_t v = i < m ? a[i] : 0u;
+    uint32_t total;
+    const uint32_t ex = block_exclusive_scan(v, ws, total);
+    if (i < m) a[i] = carry + ex;
+    carry += total;
+  }
+}
+
+// ranks of the sorted pairs -> key of every cell, the inverse table (may be null) and the key of a cell equal to nodata
+__global__ void __launch_bounds__(256) rank_scatter_kernel(const uint64_t *__restrict__ ks, const uint32_t *__restrict__ is,
+                                                           const double *__restrict__ z, size_t n,
+                                                           const uint32_t *__restrict__ sums, float *__restrict__ key,
+                                                           double *__restrict__ table, double nodata, uint32_t *nd_key) {
+  __shared__ uint32_t ws[8];
+  const HeadSrc head{ks, z};
+  const size_t base = (size_t)blockIdx.x * SORT_TILE;
+  uint32_t carry = sums[blockIdx.x];
+  int found = 0;
+  uint32_t nd_bits = 0;
+  for (int r = 0; r < SORT_ITEMS; r++) {
+    const size_t i = base + (size_t)r * SORT_THREADS + threadIdx.x;
+    const bool valid = i < n;
+    const uint32_t h = valid ? head(i) : 0u;
+    uint32_t total;
+    const uint32_t rank = carry + block_exclusive_scan(h, ws, total) + h - 1u;
+    carry += total;
+    if (valid) {
+      uint64_t k;
+      uint32_t idx;
+      load_pair(i, ks, is, z, k, idx);
+      const double v = order_value(k);
+      const float f = rank_key(v, rank);
+      key[idx] = f;
+      if (h && table) table[rank] = v;
+      if (v == nodata) {
+        found = 1;
+        nd_bits = __float_as_uint(f);
+      }
+    }
+  }
+  if (found) *nd_key = nd_bits;
+}
+
+// the fill's write-back: cells whose key the fill raised take kappa^-1 of it; the others keep their own bits
+__global__ void __launch_bounds__(256) f64_writeback_kernel(double *__restrict__ z, const float *__restrict__ key0,
+                                                            const float *__restrict__ keyf, size_t n,
+                                                            const double *__restrict__ table) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const float b = keyf[i];
+    if (__float_as_uint(b) != __float_as_uint(key0[i])) z[i] = key_value(b, table);
+  }
+}
+
+// k successive nextafter(z, +inf) on a double (flats/Barnes2014.hpp:527-528), the double twin of flats.cu's
+// advance_ulps: saturates at +inf, and a negative value that reaches zero lands on -0.0
+__device__ __forceinline__ double advance_ulps_f64(double z, int k) {
+  if (k <= 0 || z != z) return z;
+  const uint64_t b = (uint64_t)__double_as_longlong(z);
+  const bool neg = (b >> 63) != 0;
+  const long long mag = (long long)(b & 0x7fffffffffffffffull);
+  long long key = neg ? -mag : mag;  // -0.0 and +0.0 share key 0
+  key += k;
+  if (key >= 0x7ff0000000000000ll) return (double)INFINITY;
+  if (key > 0) return __longlong_as_double(key);
+  if (key == 0) return neg ? __longlong_as_double((long long)0x8000000000000000ull) : 0.0;
+  return __longlong_as_double((long long)(0x8000000000000000ull | (uint64_t)(-key)));
+}
+
+// ResolveFlatsEpsilon's apply (flats/Barnes2014.hpp:496-550) with the increment mask of the key raster: interior cells only
+__global__ void __launch_bounds__(256) f64_apply_ulps_kernel(double *__restrict__ z, const int32_t *__restrict__ mask, int W,
+                                                             int H) {
+  const size_t n = (size_t)W * H, stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int m = mask[i];
+    if (m <= 0) continue;
+    const int y = (int)(i / W), x = (int)(i - (size_t)y * W);
+    if (x > 0 && y > 0 && x < W - 1 && y < H - 1) z[i] = advance_ulps_f64(z[i], m);
+  }
+}
+
+unsigned stream_blocks(size_t n) {
+  const size_t want = (n + 255) / 256, cap = (size_t)ctx().num_sms * 8;
+  return (unsigned)(want < cap ? want : cap);
+}
+
+// d_sums[b] = the sum of src over the chunks before chunk b (nb chunks of 4096 entries of m)
+template <class Src>
+void chunk_sums_dev(Src src, size_t m, uint32_t *d_sums, size_t nb) {
+  Ctx &c = ctx();
+  chunk_sum_kernel<Src><<<(unsigned)nb, 256, 0, c.stream>>>(src, m, d_sums);
+  sums_scan_kernel<<<1, 256, 0, c.stream>>>(d_sums, nb);
+  RDB_CK(cudaGetLastError());
+  count_launch(2);
+}
+
+float host_bits_float(uint32_t b) {
+  float f;
+  memcpy(&f, &b, sizeof f);
+  return f;
+}
+
+// kappa(nodata) when no cell equals nodata
+float nodata_image(double nodata) {
+  if (nodata == (double)INFINITY) return INFINITY;
+  if (nodata == -(double)INFINITY) return -INFINITY;
+  if (nodata == DBL_MAX) return FLT_MAX;
+  if (nodata == -DBL_MAX) return -FLT_MAX;
+  return host_bits_float(0x7fc00000u);
+}
+
+}  // namespace
+
+float f64_keys_dev(const double *d_z, float *d_key, size_t n, double nodata, DevBuf<double> *table, int *ranked) {
+  Ctx &c = ctx();
+  DevBuf<uint32_t> flags(2 + 8 * 256);  // [0] inexact, [1] nodata key, [2..] digit histograms
+  uint32_t *d_inexact = flags.p, *d_nd = flags.p + 1, *d_hist = flags.p + 2;
+  RDB_CK(cudaMemsetAsync(d_inexact, 0, sizeof(uint32_t), c.stream));
+  RDB_CK(cudaMemsetAsync(d_nd, 0xff, sizeof(uint32_t), c.stream));
+  f64_cast_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, d_key, n, nodata, (int *)d_inexact, d_nd);
+  RDB_CK(cudaGetLastError());
+  count_launch();
+  uint32_t *hb = (uint32_t *)c.pinned;  // 2 + 2048 words fit the 64 KiB pinned scratch
+  RDB_CK(cudaMemcpyAsync(hb, flags.p, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  if (ranked) *ranked = hb[0] != 0;
+  if (hb[0] == 0) return hb[1] != NO_KEY ? host_bits_float(hb[1]) : nodata_image(nodata);
+
+  // case 2: which digits differ between keys
+  RDB_CK(cudaMemsetAsync(d_nd, 0xff, sizeof(uint32_t), c.stream));
+  RDB_CK(cudaMemsetAsync(d_hist, 0, 8 * 256 * sizeof(uint32_t), c.stream));
+  digit_hist_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, n, d_hist);
+  RDB_CK(cudaGetLastError());
+  count_launch();
+  RDB_CK(cudaMemcpyAsync(hb, d_hist, 8 * 256 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  int shifts[8], passes = 0;
+  for (int d = 0; d < 8; d++) {
+    uint32_t top = 0;
+    for (int b = 0; b < 256; b++) top = hb[d * 256 + b] > top ? hb[d * 256 + b] : top;
+    if (top != (uint32_t)n) shifts[passes++] = 8 * d;
+  }
+
+  const size_t tiles = (n + SORT_TILE - 1) / SORT_TILE;
+  DevBuf<uint64_t> ka, kb;
+  DevBuf<uint32_t> ia, ib, counts, sums;
+  sums.alloc(tiles);  // chunk sums: n / 4096 chunks of run heads, 256 * tiles / 4096 of tile counts
+  if (passes) {
+    ka.alloc(n), kb.alloc(n), ia.alloc(n), ib.alloc(n), counts.alloc(256 * tiles);
+  }
+  const uint64_t *ks = nullptr;
+  const uint32_t *is = nullptr;
+  const double *zsrc = d_z;  // the first pass reads Z itself
+  for (int p = 0; p < passes; p++) {
+    uint64_t *ko = (p & 1) ? kb.p : ka.p;
+    uint32_t *io = (p & 1) ? ib.p : ia.p;
+    const size_t m = 256 * tiles, nb = (m + SORT_TILE - 1) / SORT_TILE;
+    tile_count_kernel<<<(unsigned)tiles, 256, 0, c.stream>>>(ks, zsrc, n, shifts[p], counts.p, (uint32_t)tiles);
+    chunk_sums_dev(ArraySrc{counts.p}, m, sums.p, nb);
+    scan_apply_kernel<<<(unsigned)nb, 256, 0, c.stream>>>(counts.p, m, sums.p);
+    tile_scatter_kernel<<<(unsigned)tiles, 256, 0, c.stream>>>(ks, is, zsrc, ko, io, n, shifts[p], counts.p, (uint32_t)tiles);
+    RDB_CK(cudaGetLastError());
+    count_launch(3);
+    ks = ko, is = io, zsrc = nullptr;
+  }
+  counts.reset();
+  if (table) table->alloc(n);
+  chunk_sums_dev(HeadSrc{ks, zsrc}, n, sums.p, tiles);
+  rank_scatter_kernel<<<(unsigned)tiles, 256, 0, c.stream>>>(ks, is, zsrc, n, sums.p, d_key, table ? table->p : nullptr, nodata,
+                                                             d_nd);
+  RDB_CK(cudaGetLastError());
+  count_launch();
+  RDB_CK(cudaMemcpyAsync(hb, d_nd, sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  return hb[0] != NO_KEY ? host_bits_float(hb[0]) : nodata_image(nodata);
+}
+
+// FillDepressions<D8 / D4> of a double raster: fill the key raster, then write kappa^-1 of every raised key
+void fill_depressions_f64_dev(double *d_z, int w, int h, bool topo4) {
+  Ctx &c = ctx();
+  const size_t n = (size_t)w * h;
+  DevBuf<float> k0(n), kf(n);
+  DevBuf<double> table;
+  f64_keys_dev(d_z, k0.p, n, 0.0, &table, nullptr);
+  RDB_CK(cudaMemcpyAsync(kf.p, k0.p, n * sizeof(float), cudaMemcpyDeviceToDevice, c.stream));
+  fill_depressions_dev(kf.p, w, h, topo4);
+  f64_writeback_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, k0.p, kf.p, n, table.p);
+  RDB_CK(cudaGetLastError());
+  count_launch();
+  c.stats.cells = (int64_t)n;
+}
+
+void pit_mask_f64_dev(const double *d_z, uint8_t *d_mask, int w, int h, double nodata, bool topo4) {
+  Ctx &c = ctx();
+  const size_t n = (size_t)w * h;
+  DevBuf<float> k0(n), kf(n);
+  DevBuf<int> any(1);
+  const float nd = f64_keys_dev(d_z, k0.p, n, nodata, nullptr, nullptr);
+  RDB_CK(cudaMemsetAsync(any.p, 0, sizeof(int), c.stream));
+  RDB_CK(cudaMemcpyAsync(kf.p, k0.p, n * sizeof(float), cudaMemcpyDeviceToDevice, c.stream));
+  fill_depressions_dev(kf.p, w, h, topo4);
+  pit_mask_compare_dev(k0.p, kf.p, d_mask, n, nd, any.p);
+  c.stats.cells = (int64_t)n;
+}
+
+bool has_depressions_f64_dev(const double *d_z, int w, int h, bool topo4) {
+  Ctx &c = ctx();
+  const size_t n = (size_t)w * h;
+  DevBuf<int> flag(1);
+  RDB_CK(cudaMemsetAsync(flag.p, 0, sizeof(int), c.stream));
+  strict_pit_f64_dev(d_z, w, h, topo4, flag.p);
+  int *hf = (int *)c.pinned;
+  RDB_CK(cudaMemcpyAsync(hf, flag.p, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  if (*hf) return true;
+  if (w < 3 || h < 3) return false;  // every cell is an edge cell
+  DevBuf<float> k0(n), kf(n);
+  f64_keys_dev(d_z, k0.p, n, 0.0, nullptr, nullptr);
+  RDB_CK(cudaMemcpyAsync(kf.p, k0.p, n * sizeof(float), cudaMemcpyDeviceToDevice, c.stream));
+  fill_depressions_dev(kf.p, w, h, topo4);
+  pit_mask_compare_dev(k0.p, kf.p, nullptr, n, 0.f, flag.p);
+  RDB_CK(cudaMemcpyAsync(hf, flag.p, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  c.stats.cells = (int64_t)n;
+  return *hf != 0;
+}
+
+// ResolveFlatsEpsilon: the increment mask of the key raster (GetFlatMask), applied as double ulps to the original values
+void resolve_flats_f64_dev(double *d_z, int w, int h, double nodata) {
+  Ctx &c = ctx();
+  const size_t n = (size_t)w * h;
+  DevBuf<float> key(n);
+  const float nd = f64_keys_dev(d_z, key.p, n, nodata, nullptr, nullptr);
+  DevBuf<int32_t> mask(n);
+  resolve_flats_dev(key.p, w, h, nd, mask.p, nullptr, false);
+  f64_apply_ulps_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, mask.p, w, h);
+  RDB_CK(cudaGetLastError());
+  count_launch();
+}
+
+// FA_D8 (unit or given weights) on the key raster: the accumulation carries no elevation values
+void fa_d8_f64_dev(const double *d_z, double *d_accum, int w, int h, double nodata, bool ones) {
+  const size_t n = (size_t)w * h;
+  DevBuf<float> key(n);
+  const float nd = f64_keys_dev(d_z, key.p, n, nodata, nullptr, nullptr);
+  fa_fused_dev(key.p, d_accum, w, h, nd, ones, false);
+}
+
+}  // namespace rdb

@@ -13,14 +13,14 @@ namespace rdb {
 
 namespace {
 
-// d8_FlowDir, flowmet/d8_flowdirs.hpp:32-74
-__global__ void d8_flowdirs_kernel(const float *__restrict__ dem, uint8_t *__restrict__ dirs, int W, int H,
-                                   float nodata) {
+// d8_FlowDir, flowmet/d8_flowdirs.hpp:32-74; T is float, or double for rdb200_d8_flow_directions_f64
+template <class T>
+__global__ void d8_flowdirs_kernel(const T *__restrict__ dem, uint8_t *__restrict__ dirs, int W, int H, T nodata) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x;
   if (x >= W) return;
   for (int y = blockIdx.y; y < H; y += gridDim.y) {
     const size_t i = (size_t)y * W + x;
-    const float e = __ldg(dem + i);
+    const T e = __ldg(dem + i);
     uint8_t d;
     if (e == nodata) {  // :117-118
       d = 255;
@@ -34,11 +34,11 @@ __global__ void d8_flowdirs_kernel(const float *__restrict__ dem, uint8_t *__res
       else if (y == 0) d = 3;
       else d = 7;
     } else {
-      float minimum = e;
+      T minimum = e;
       int flowdir = 0;
 #pragma unroll
       for (int n = 1; n <= 8; n++) {  // :63-71 (NoData neighbours are NOT skipped here)
-        const float ne = __ldg(dem + (size_t)(y + d8dy(n)) * W + (x + d8dx(n)));
+        const T ne = __ldg(dem + (size_t)(y + d8dy(n)) * W + (x + d8dx(n)));
         if (ne < minimum || (ne == minimum && flowdir > 0 && (flowdir & 1) == 0 && (n & 1) == 1)) {
           minimum = ne;
           flowdir = n;
@@ -214,8 +214,17 @@ void d8_flow_directions_dev(const float *d_dem, uint8_t *d_dirs, int w, int h, f
     d8_flowdirs_rolling_kernel<<<grd, blk, 0, c.stream>>>(d_dem, d_dirs, w, h, nodata);
   } else {
     dim3 blk(128), grd((w + 127) / 128, h < 16384 ? h : 16384);
-    d8_flowdirs_kernel<<<grd, blk, 0, c.stream>>>(d_dem, d_dirs, w, h, nodata);
+    d8_flowdirs_kernel<float><<<grd, blk, 0, c.stream>>>(d_dem, d_dirs, w, h, nodata);
   }
+  RDB_CK(cudaGetLastError());
+  count_launch();
+}
+
+// the same rule on doubles, compared as doubles (one 8 B load per cell and neighbour, 1 B out)
+void d8_flow_directions_f64_dev(const double *d_dem, uint8_t *d_dirs, int w, int h, double nodata) {
+  Ctx &c = ctx();
+  dim3 blk(128), grd((w + 127) / 128, h < 16384 ? h : 16384);
+  d8_flowdirs_kernel<double><<<grd, blk, 0, c.stream>>>(d_dem, d_dirs, w, h, nodata);
   RDB_CK(cudaGetLastError());
   count_launch();
 }
