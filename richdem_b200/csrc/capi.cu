@@ -252,6 +252,7 @@ int rdb200_set_param(const char *name, int64_t value) {
   else if (n == "fill_use_tma") p.fill_use_tma = value;
   else if (n == "fill_external_z") p.fill_external_z = value;
   else if (n == "fill_profile") p.fill_profile = value;
+  else if (n == "fill_wake_filter") p.fill_wake_filter = value;
   else if (n == "fill_trace") p.fill_trace = value;
   else if (n == "fill_ordered") p.fill_ordered = value;
   else if (n == "fill_order_rounds") p.fill_order_rounds = value;

@@ -62,6 +62,7 @@ struct Params {
   int64_t fill_order_rounds = 0;  // rounds the level schedule spans (0: 0.8 x tiles across the raster)
   int64_t fill_band_rounds = 0;   // row-band mode: rounds per rdb200_dev_fill_run call (0: to convergence)
   int64_t fill_profile = 0;     // 1: collect + print in-tile work counters (slower)
+  int64_t fill_wake_filter = 1; // fill: wake a neighbouring tile only when the new edge can lower one of its cells (0: always)
   int64_t fill_trace = 0;       // 1: per-V-cycle timeline of the multigrid fill on stderr (adds stream syncs)
   int64_t fill_multigrid = 8;      // k >= 2: start the flood from the lifted fill of the k x k max-pooled raster (recursive)
   int64_t fill_vcycle = 8;         // with fill_multigrid: coarse-grid correction after every that many fine rounds (0: none)

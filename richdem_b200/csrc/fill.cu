@@ -71,6 +71,7 @@ struct FillDev {
   unsigned long long block_updates;  // 4x4 blocks relaxed (threads that did not skip a pass)
   unsigned long long warp_updates;   // warps with at least one such thread
   unsigned long long idle_visits;    // tile visits that changed nothing
+  unsigned long long wakes_dropped;  // changed tile sides / corners whose neighbour the wake test left asleep
   unsigned long long iter_hist[8];   // visits by pass count: 1,2,3-4,5-8,9-16,17-32,33-64,65+
   int edge_changed;  // bit0: raster row 1 changed, bit1: raster row H-2 changed
   int zmin_ord, zmax_ord;  // ordered-int min / max of the finite input elevations
@@ -114,6 +115,9 @@ struct FillArgs {
   int use_tma;
   int profile;
   int *dirty;  // per tile: a visit wrote cells back since the flags were last cleared (V-cycle bookkeeping; may be null)
+  // fill only (null: every changed side wakes its neighbour): per tile, one word per edge line -- N row, S row, W column,
+  // E column -- with bit i set while cell i of that line may still be above its Z (see fill_wake_neighbours)
+  unsigned long long *edge_above;
 };
 
 // ---- PTX helpers: mbarrier + TMA ----------------------------------------------------------
@@ -208,6 +212,42 @@ __device__ __forceinline__ void enqueue_tile(const FillArgs &a, RoundCtl *next, 
 
 __device__ __forceinline__ float min3f(float a, float b, float c) { return fminf(fminf(a, b), c); }
 
+// ---- the wake test (fill only) ----------------------------------------------------------------------------------------
+// A changed tile edge used to wake the neighbour across it whatever the new values were, and most of those visits found
+// nothing to do: the neighbour's cell next to the edge already sat at its Z (W == Z never moves again) or at or below
+// the new edge.  Now the neighbour N across a changed side or corner is only woken if one of its cells `a` next to the
+// edge has
+//     its bit set in N's edge_above word   and   min(this tile's own cells adjacent to a) < W(a),
+// i.e. if the new edge can lower a.  W(a) is taken from this visit's apron: the copy of N's cells the visit started from.
+// No fence protocol is needed:
+//   * N's cells only decrease, so the apron value is at least every value N holds now or later -- whether N is idle or
+//     in a visit of its own (each cell read before or after N's store of it): e >= W_apron(a) means the new edge
+//     cannot lower a in either case;
+//   * a bit is cleared only for a cell at W == Z, which relaxation never moves again (Z only changes on the ghost rows
+//     of a row band, border cells whose W drops with it), so a stale word only has bits set that could be clear: an
+//     extra wake, never a lost one;
+//   * when N is woken, its visit in the next launch sees this tile's stores.
+// The staged first round needs no exception: the apron of a neighbour that had not stored its cells when the window was
+// built holds the lifted level that neighbour starts from -- never the raster's Z, which is below it -- and so bounds
+// every value the neighbour stores from above; a tile's words read all ones until its first visit stores them.
+// Only the tile's own cells count (three for D8, one for D4; one against one at a corner, and no D4 corner wake: that
+// stencil never reads the corner aprons): an apron cell belongs to another tile, which tests its own edge.
+constexpr bool WAKE_WORDS = TX <= 64 && TY <= 64;  // one 64-bit word per edge line
+
+// edge line s of the W window (0: N row, 1: S row, 2: W column, 3: E column): cell i at sW[o + i * st], the neighbour's
+// adjacent cell at sW[o + i * st + da], its Z at sZ[zo + i * zs]
+struct EdgeLine {
+  int len, o, st, da, zo, zs;
+};
+__device__ __forceinline__ EdgeLine edge_line(int s) {
+  switch (s) {
+    case 0: return {TX, SP + PADL, 1, -SP, 0, 1};
+    case 1: return {TX, TY * SP + PADL, 1, SP, (TY - 1) * TX, 1};
+    case 2: return {TY, SP + PADL, SP, -1, 0, TX};
+    default: return {TY, SP + PADL + TX - 1, SP, 1, TX - 1, TX};
+  }
+}
+
 // ---- staged first round: drain the lifted tile with column sweeps -----------------------------------------------------
 // A tile of the staged round starts from the lifted surface (constant pool x pool plateaus) and must drain nearly every
 // cell down towards Z, with all of its blocks dirty.  Before the dirty-block relaxation (which then runs unchanged from
@@ -285,6 +325,66 @@ __device__ __forceinline__ void fill_drain_sweeps(float *sW, const float *sZ, in
   // (the second half's __syncthreads above already published the swept window to the block loop)
 }
 
+// End of a fill visit (sW / sZ: the relaxed window; fl: the tile's change flags, key: the lowest new edge level): store
+// the tile's edge words, then wake the neighbours across the changed sides and corners that the new edge can lower.
+// One warp per edge line; lane 1 of warp s takes corner s (NW, NE, SW, SE).
+#ifndef __noinline__
+#define __noinline__ __attribute__((noinline))
+#endif
+template <bool TOPO4>
+__device__ __noinline__ void fill_wake_neighbours(const FillArgs &a, const float *sW, const float *sZ, int t, int fl, int key,
+                                                  RoundCtl *next, int *list_next) {
+  const unsigned FULL = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const int tyT = t / a.tilesX, txT = t - tyT * a.tilesX;
+  const bool n_ok = tyT > 0, s_ok = tyT < a.tilesY - 1, w_ok = txT > 0, e_ok = txT < a.tilesX - 1;
+  const int sv = a.round + 1;
+  for (int s = threadIdx.x >> 5; s < 4; s += NWARP) {
+    const EdgeLine e = edge_line(s);
+    unsigned long long word = 0;
+    for (int i0 = 0; i0 < e.len; i0 += 32) {
+      const int i = i0 + lane;
+      const bool above = i < e.len && !(sW[e.o + i * e.st] == sZ[e.zo + i * e.zs]);
+      word |= (unsigned long long)__ballot_sync(FULL, above) << i0;
+    }
+    if (lane == 0) __stcg(&a.edge_above[(size_t)t * 4 + s], word);
+    if (!((fl >> 12) & 0xFFFF)) continue;  // nothing changed (warp-uniform)
+    if (!TOPO4 && lane == 1 && (fl & (SIDE_NW << s))) {
+      // corner s: this tile's corner cell against the diagonal neighbour's, the first or last bit of that neighbour's
+      // row next to this tile
+      const bool north = s < 2, west = (s & 1) == 0;
+      if ((north ? n_ok : s_ok) && (west ? w_ok : e_ok)) {
+        const int nb = t + (north ? -a.tilesX : a.tilesX) + (west ? -1 : 1);
+        const int own = (north ? SP : TY * SP) + PADL + (west ? 0 : TX - 1);
+        const int across = own + (north ? -SP : SP) + (west ? -1 : 1);
+        const unsigned long long nword = __ldcg(&a.edge_above[(size_t)nb * 4 + (north ? 1 : 0)]);
+        if (((nword >> (west ? TX - 1 : 0)) & 1ull) && sW[own] < sW[across])
+          enqueue_tile(a, next, list_next, nb, sv, SIDE_NW << (3 - s), key);
+        else if (a.profile)
+          atomicAdd(&a.dev->wakes_dropped, 1ull);
+      }
+    }
+    if (!((fl >> s) & 1) || !(s == 0 ? n_ok : s == 1 ? s_ok : s == 2 ? w_ok : e_ok)) continue;  // (warp-uniform)
+    const int nb = s == 0 ? t - a.tilesX : s == 1 ? t + a.tilesX : s == 2 ? t - 1 : t + 1;
+    const unsigned long long nword = __ldcg(&a.edge_above[(size_t)nb * 4 + (s ^ 1)]);  // its line next to this tile
+    bool need = false;
+    for (int i = lane; i < e.len; i += 32) {
+      if (!((nword >> i) & 1ull)) continue;
+      float m = sW[e.o + i * e.st];
+      if (!TOPO4) {
+        if (i > 0) m = fminf(m, sW[e.o + (i - 1) * e.st]);
+        if (i < e.len - 1) m = fminf(m, sW[e.o + (i + 1) * e.st]);
+      }
+      need |= m < sW[e.o + i * e.st + e.da];
+    }
+    if (__ballot_sync(FULL, need)) {
+      if (lane == 0) enqueue_tile(a, next, list_next, nb, sv, 1 << (s ^ 1), key);
+    } else if (lane == 0 && a.profile) {
+      atomicAdd(&a.dev->wakes_dropped, 1ull);
+    }
+  }
+}
+
 // STEP = 0: depression filling,     new = min(W, max(Z, min8 W))
 // STEP = 1: geodesic distance,      new = min(W, max(Z, 1 + min8 W))   with Z = 0 on cells the flood
 //           may enter and +inf elsewhere (used for the flat-resolution gradients, csrc/flats.cu)
@@ -295,7 +395,7 @@ __device__ __forceinline__ void fill_drain_sweeps(float *sW, const float *sZ, in
 template <int STEP, bool TOPO4 = false, bool STAGE = false>
 __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
     fill_sweep_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__ CUtensorMap mapZ,
-                      const __grid_constant__ CUtensorMap mapZout, const FillArgs a) {
+                      const __grid_constant__ CUtensorMap mapZout, const __grid_constant__ FillArgs a) {
   __shared__ __align__(128) float sW[SROWS * SP];
   __shared__ __align__(128) float sZ[TY * TX];
   __shared__ __align__(8) unsigned long long mbar;
@@ -508,7 +608,14 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
         atomicExch(&a.staged[t], 1);
       }
     }
-    if (rowch) {
+    if (STEP == 0 && WAKE_WORDS && a.edge_above) {
+      // (not inlined: the relaxation above keeps its registers)
+      fill_wake_neighbours<TOPO4>(a, sW, sZ, t, fl, sKey, next, list_next);
+      if (rowch && tid == 0) {
+        if (fl & (3 << 9)) atomicOr(&a.dev->edge_changed, (fl >> 9) & 3);
+        if (a.dirty) a.dirty[t] = 1;
+      }
+    } else if (rowch) {
       if (tid < 8) {
         // one thread per neighbour: the enqueue atomics (or + exch + add) overlap instead of
         // queueing behind each other on a single thread
@@ -1000,6 +1107,7 @@ struct FillState {
   DevBuf<int> list0, list1, plist, stamp, sides, keys;
   DevBuf<int> dirty, tflag;  // V-cycle bookkeeping: tiles written since the last look / tiles to wake (both per tile)
   DevBuf<int> staged;        // staged lifted start: tiles the first round has written (per tile)
+  DevBuf<unsigned long long> edge_above;  // fill: 4 words per tile for the wake test (FillArgs::edge_above)
   float zmin = 0.f, zmax = 0.f;
   bool first_run = true;
   bool ordered = false;
@@ -1082,6 +1190,10 @@ struct FillState {
       staged.alloc(nt);
       RDB_CK(cudaMemsetAsync(staged.p, 0, nt * sizeof(int), c.stream));
     }
+    // every cell may be above its Z until its tile's first visit says otherwise (whatever the start: +inf, lifted in
+    // place or padded, staged, a band's, fill_relax_from's)
+    edge_above.alloc(4 * nt);
+    RDB_CK(cudaMemsetAsync(edge_above.p, 0xff, 4 * nt * sizeof(unsigned long long), c.stream));
     {
       FillDev h0;
       memset(&h0, 0, sizeof(h0));
@@ -1281,6 +1393,8 @@ struct FillState {
     a.profile = (int)c.params.fill_profile;
     a.level = __builtin_inff();
     a.dirty = dirty.p;  // null unless track_dirty() was called
+    // (the distance mode wakes every neighbour across a changed side, as the fill does with fill_wake_filter = 0)
+    a.edge_above = step_mode == 0 && c.params.fill_wake_filter != 0 ? edge_above.p : nullptr;
     return a;
   }
 
@@ -1366,14 +1480,21 @@ struct FillState {
     c.stats.fill_tile_iters = iters_seen;
     c.stats.fill_tile_cells = TX * TY;
     if (c.params.fill_profile) {
-      fprintf(stderr, "[fill profile] deferred=%llu visits=%llu iters=%llu block_updates=%llu (%.1f%% of 256/iter) warp_updates=%llu (%.1f%% of 8/iter) idle_visits=%llu hist(1,2,3-4,5-8,9-16,17-32,33-64,65+)=",
+      fprintf(stderr, "[fill profile] deferred=%llu visits=%llu iters=%llu block_updates=%llu (%.1f%% of 256/iter) warp_updates=%llu (%.1f%% of 8/iter) idle_visits=%llu wakes_dropped=%llu hist(1,2,3-4,5-8,9-16,17-32,33-64,65+)=",
               hd->deferred, hd->visits, hd->iters, hd->block_updates, 100.0 * hd->block_updates / (256.0 * hd->iters + 1),
-              hd->warp_updates, 100.0 * hd->warp_updates / (8.0 * hd->iters + 1), hd->idle_visits);
+              hd->warp_updates, 100.0 * hd->warp_updates / (8.0 * hd->iters + 1), hd->idle_visits, hd->wakes_dropped);
       for (int k = 0; k < 8; k++) fprintf(stderr, "%llu ", hd->iter_hist[k]);
       fprintf(stderr, "\n");
+      // what this run added, so that the lines of all the solvers of a call (coarse levels, V-cycle corrections) sum
+      fprintf(stderr, "[fill wake] visits=%llu idle_visits=%llu wakes_dropped=%llu\n", hd->visits - prof_seen[0],
+              hd->idle_visits - prof_seen[1], hd->wakes_dropped - prof_seen[2]);
+      prof_seen[0] = hd->visits;
+      prof_seen[1] = hd->idle_visits;
+      prof_seen[2] = hd->wakes_dropped;
     }
     return batch_edge | (still_active ? 4 : 0);
   }
+  unsigned long long prof_seen[3] = {0, 0, 0};  // fill_profile: visits, idle visits, dropped wakes reported so far
 
   // V-cycle plumbing (fill_vcycle): see fill_depressions_level
   void track_dirty() {  // from now on the sweep notes which tiles it wrote
