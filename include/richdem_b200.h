@@ -252,6 +252,34 @@ RDB200_API int rdb200_fa_d8_f32_f64(const float *dem, double *accum_inout, int32
 RDB200_API int rdb200_fa_tarboton_f32_f64(const float *dem, double *accum_inout, int32_t width,
                                int32_t height, float nodata, int32_t accum_is_ones);
 
+/* float64 elevations for the stages that do arithmetic on them: the reference's templates with E / T = double, run by
+ * the double instantiations of the float kernels (no keys).  Arguments, checks and tolerances as the float entry points
+ * above; NoData is a double.  s1, s2, e0 - e2 (D-infinity) and e - ne (Holmgren, Freeman) are rounded double
+ * differences, as in the reference; DESIGN §0.2 gives the D-infinity fallback for differences outside [2^-500, 2^500].
+ *   fm_*_f64                 flowmet/OCallaghan1984.hpp, Tarboton1997.hpp, Quinn1991.hpp, Holmgren1994.hpp, Freeman1991.hpp
+ *   fa_tarboton_f64_f64      methods/flow_accumulation.hpp:16 (FA_Tarboton<double, double>): the fused engine of
+ *                            rdb200_fa_tarboton_f32_f64 after a code pass on the doubles; accum_is_ones as there
+ *   fa_{quinn,holmgren,freeman}_f64_f64  methods/flow_accumulation.hpp:18-20: FM_x on the doubles + the generic
+ *                            accumulation; accum_inout holds the weights
+ *   terrain_attribute_f64    methods/terrain_attributes.hpp:370-538 with T = double; float output */
+RDB200_API int rdb200_fm_d8_f64(const double *dem, float *props9, int32_t width, int32_t height, double nodata);
+RDB200_API int rdb200_fm_tarboton_f64(const double *dem, float *props9, int32_t width, int32_t height, double nodata);
+RDB200_API int rdb200_fm_d4_f64(const double *dem, float *props9, int32_t width, int32_t height, double nodata);
+RDB200_API int rdb200_fm_quinn_f64(const double *dem, float *props9, int32_t width, int32_t height, double nodata);
+RDB200_API int rdb200_fm_holmgren_f64(const double *dem, float *props9, int32_t width, int32_t height, double nodata,
+                                      double xparam);
+RDB200_API int rdb200_fm_freeman_f64(const double *dem, float *props9, int32_t width, int32_t height, double nodata,
+                                     double xparam);
+RDB200_API int rdb200_fa_tarboton_f64_f64(const double *dem, double *accum_inout, int32_t width, int32_t height,
+                                          double nodata, int32_t accum_is_ones);
+RDB200_API int rdb200_fa_quinn_f64_f64(const double *dem, double *accum_inout, int32_t width, int32_t height, double nodata);
+RDB200_API int rdb200_fa_holmgren_f64_f64(const double *dem, double *accum_inout, int32_t width, int32_t height,
+                                          double nodata, double xparam);
+RDB200_API int rdb200_fa_freeman_f64_f64(const double *dem, double *accum_inout, int32_t width, int32_t height,
+                                         double nodata, double xparam);
+RDB200_API int rdb200_terrain_attribute_f64(int32_t attribute, const double *dem, float *out, int32_t width, int32_t height,
+                                            double nodata_in, float nodata_out, float zscale, double cell_x, double cell_y);
+
 /* ---- device entry points (pointers into HBM of the current device) ----------------- */
 
 /* Depression filling in place.  While the call runs, d_dem holds intermediate water levels (when width is a multiple
@@ -304,6 +332,17 @@ RDB200_API int rdb200_dev_fa_d8_f64_f64(const double *d_dem, double *d_accum_ino
                                         double nodata, int32_t accum_is_ones);
 RDB200_API int rdb200_dev_fa_d4_f64_f64(const double *d_dem, double *d_accum_inout, int32_t width, int32_t height,
                                         double nodata);
+/* method numbered as in rdb200_dev_fm_method_f32; rdb200_dev_fa_method_f64_f64 runs methods 0 and 2 as
+ * rdb200_dev_fa_d8_f64_f64 (given weights) and rdb200_dev_fa_d4_f64_f64, the others through proportions */
+RDB200_API int rdb200_dev_fm_method_f64(int32_t method, const double *d_dem, float *d_props9, int32_t width, int32_t height,
+                                        double nodata, double xparam);
+RDB200_API int rdb200_dev_fa_method_f64_f64(int32_t method, const double *d_dem, double *d_accum_inout, int32_t width,
+                                            int32_t height, double nodata, double xparam);
+RDB200_API int rdb200_dev_fa_tarboton_f64_f64(const double *d_dem, double *d_accum_inout, int32_t width, int32_t height,
+                                              double nodata, int32_t accum_is_ones);
+RDB200_API int rdb200_dev_terrain_attribute_f64(int32_t attribute, const double *d_dem, float *d_out, int32_t width,
+                                                int32_t height, double nodata_in, float nodata_out, float zscale,
+                                                double cell_x, double cell_y);
 /* diagnostic, as rdb200_f64_order_keys */
 RDB200_API int rdb200_dev_f64_order_keys(const double *d_dem, float *d_keys, int32_t width, int32_t height, double nodata,
                                          float *nodata_key, int32_t *ranked);

@@ -428,6 +428,84 @@ inline void FA_D4<double, double>(const Array2D<double> &elevations, Array2D<dou
   richdem_b200::check(rdb200_fa_d4_f64_f64(elevations.data(), accum.data(), elevations.width(), elevations.height(),
                                            elevations.noData()));
 }
+// flowmet/OCallaghan1984.hpp:81-91, Tarboton1997.hpp:14-149, Quinn1991.hpp:12-16, Holmgren1994.hpp:13-83,
+// Freeman1991.hpp:13-80 with E = double: the double instantiations of the float kernels (no keys; DESIGN §0.2)
+#define RICHDEM_B200_FM64(NAME, CALL)                                                                          \
+  template <>                                                                                                 \
+  inline void NAME<double>(const Array2D<double> &elevations, Array3D<float> &props) {                        \
+    props.setNoData(NO_DATA_GEN);                                                                             \
+    richdem_b200::check(CALL(elevations.data(), props.getData(), elevations.width(), elevations.height(),     \
+                             elevations.noData()));                                                           \
+  }
+RICHDEM_B200_FM64(FM_D8, rdb200_fm_d8_f64)
+RICHDEM_B200_FM64(FM_D4, rdb200_fm_d4_f64)
+RICHDEM_B200_FM64(FM_Tarboton, rdb200_fm_tarboton_f64)
+RICHDEM_B200_FM64(FM_Dinfinity, rdb200_fm_tarboton_f64)
+RICHDEM_B200_FM64(FM_Quinn, rdb200_fm_quinn_f64)
+#undef RICHDEM_B200_FM64
+template <>
+inline void FM_Holmgren<double>(const Array2D<double> &elevations, Array3D<float> &props, const double xparam) {
+  props.setNoData(NO_DATA_GEN);
+  richdem_b200::check(rdb200_fm_holmgren_f64(elevations.data(), props.getData(), elevations.width(), elevations.height(),
+                                             elevations.noData(), xparam));
+}
+template <>
+inline void FM_Freeman<double>(const Array2D<double> &elevations, Array3D<float> &props, const double xparam) {
+  props.setNoData(NO_DATA_GEN);
+  richdem_b200::check(rdb200_fm_freeman_f64(elevations.data(), props.getData(), elevations.width(), elevations.height(),
+                                            elevations.noData(), xparam));
+}
+// methods/flow_accumulation.hpp:16-20 with E = double; accum holds the weights, as for float
+#define RICHDEM_B200_FA64(NAME, CALL)                                                                          \
+  template <>                                                                                                 \
+  inline void NAME<double, double>(const Array2D<double> &elevations, Array2D<double> &accum) {               \
+    accum.setNoData(ACCUM_NO_DATA);                                                                           \
+    if (accum.width() != elevations.width() || accum.height() != elevations.height())                         \
+      throw std::runtime_error("Accumulation array must have same dimensions as proportions array!");         \
+    CALL;                                                                                                     \
+  }
+RICHDEM_B200_FA64(FA_Tarboton, richdem_b200::check(rdb200_fa_tarboton_f64_f64(elevations.data(), accum.data(),
+                  elevations.width(), elevations.height(), elevations.noData(), 0)))
+RICHDEM_B200_FA64(FA_Dinfinity, richdem_b200::check(rdb200_fa_tarboton_f64_f64(elevations.data(), accum.data(),
+                  elevations.width(), elevations.height(), elevations.noData(), 0)))
+RICHDEM_B200_FA64(FA_Quinn, richdem_b200::check(rdb200_fa_quinn_f64_f64(elevations.data(), accum.data(),
+                  elevations.width(), elevations.height(), elevations.noData())))
+#undef RICHDEM_B200_FA64
+template <>
+inline void FA_Holmgren<double, double>(const Array2D<double> &elevations, Array2D<double> &accum, double xparam) {
+  accum.setNoData(ACCUM_NO_DATA);
+  if (accum.width() != elevations.width() || accum.height() != elevations.height())
+    throw std::runtime_error("Accumulation array must have same dimensions as proportions array!");
+  richdem_b200::check(rdb200_fa_holmgren_f64_f64(elevations.data(), accum.data(), elevations.width(), elevations.height(),
+                                                 elevations.noData(), xparam));
+}
+template <>
+inline void FA_Freeman<double, double>(const Array2D<double> &elevations, Array2D<double> &accum, double xparam) {
+  accum.setNoData(ACCUM_NO_DATA);
+  if (accum.width() != elevations.width() || accum.height() != elevations.height())
+    throw std::runtime_error("Accumulation array must have same dimensions as proportions array!");
+  richdem_b200::check(rdb200_fa_freeman_f64_f64(elevations.data(), accum.data(), elevations.width(), elevations.height(),
+                                                elevations.noData(), xparam));
+}
+// methods/terrain_attributes.hpp:370-538 with T = double; as for float the output is resized and keeps its own NoData
+#define RICHDEM_B200_TA64(NAME, ID)                                                                            \
+  template <>                                                                                                 \
+  inline void NAME<double>(const Array2D<double> &elevations, Array2D<float> &output, float zscale) {         \
+    output.resize(elevations);                                                                                \
+    richdem_b200::check(rdb200_terrain_attribute_f64(ID, elevations.data(), output.data(), elevations.width(), \
+                                                     elevations.height(), elevations.noData(), output.noData(), \
+                                                     zscale, elevations.getCellLengthX(),                     \
+                                                     elevations.getCellLengthY()));                           \
+  }
+RICHDEM_B200_TA64(TA_slope_riserun, RDB200_TA_SLOPE_RISERUN)
+RICHDEM_B200_TA64(TA_slope_percentage, RDB200_TA_SLOPE_PERCENTAGE)
+RICHDEM_B200_TA64(TA_slope_degrees, RDB200_TA_SLOPE_DEGREES)
+RICHDEM_B200_TA64(TA_slope_radians, RDB200_TA_SLOPE_RADIANS)
+RICHDEM_B200_TA64(TA_aspect, RDB200_TA_ASPECT)
+RICHDEM_B200_TA64(TA_curvature, RDB200_TA_CURVATURE)
+RICHDEM_B200_TA64(TA_planform_curvature, RDB200_TA_PLANFORM_CURVATURE)
+RICHDEM_B200_TA64(TA_profile_curvature, RDB200_TA_PROFILE_CURVATURE)
+#undef RICHDEM_B200_TA64
 #endif  // RICHDEM_B200_F64
 
 }  // namespace richdem

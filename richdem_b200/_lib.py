@@ -110,6 +110,21 @@ SIGNATURES = {
     "rdb200_dev_fa_d8_f64_f64": [_vp, _vp, _i32, _i32, _f64, _i32],
     "rdb200_dev_fa_d4_f64_f64": [_vp, _vp, _i32, _i32, _f64],
     "rdb200_dev_f64_order_keys": [_vp, _vp, _i32, _i32, _f64, C.POINTER(_f32), C.POINTER(_i32)],
+    "rdb200_fm_d8_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_fm_tarboton_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_fm_d4_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_fm_quinn_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_fm_holmgren_f64": [_vp, _vp, _i32, _i32, _f64, _f64],
+    "rdb200_fm_freeman_f64": [_vp, _vp, _i32, _i32, _f64, _f64],
+    "rdb200_fa_tarboton_f64_f64": [_vp, _vp, _i32, _i32, _f64, _i32],
+    "rdb200_fa_quinn_f64_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_fa_holmgren_f64_f64": [_vp, _vp, _i32, _i32, _f64, _f64],
+    "rdb200_fa_freeman_f64_f64": [_vp, _vp, _i32, _i32, _f64, _f64],
+    "rdb200_terrain_attribute_f64": [_i32, _vp, _vp, _i32, _i32, _f64, _f32, _f32, _f64, _f64],
+    "rdb200_dev_fm_method_f64": [_i32, _vp, _vp, _i32, _i32, _f64, _f64],
+    "rdb200_dev_fa_method_f64_f64": [_i32, _vp, _vp, _i32, _i32, _f64, _f64],
+    "rdb200_dev_fa_tarboton_f64_f64": [_vp, _vp, _i32, _i32, _f64, _i32],
+    "rdb200_dev_terrain_attribute_f64": [_i32, _vp, _vp, _i32, _i32, _f64, _f32, _f32, _f64, _f64],
     "rdb200_dev_generate_fbm_f32": [_vp, _i32, _i32, _i32, C.c_uint32, _i32, _f32],
     "rdb200_nccl_unique_id": [_vp],
     "rdb200_comm_create_nccl": [C.POINTER(_vp), _i32, _i32, _vp],

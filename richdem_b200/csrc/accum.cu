@@ -28,10 +28,11 @@ constexpr int kCodeSource = 64;  // bit 6: this cell has no donors (set by the f
 constexpr int kLaneChunk = 1024;  // cells a persistent warp fetches per cursor atomic (source scans)
 
 // ---- K1: dem -> compact flow code (+ rmax for D-infinity), weights/NoData initialisation ------
-template <bool DINF>
-__global__ void __launch_bounds__(256) flow_code_kernel(const float *__restrict__ dem, uint8_t *__restrict__ code,
+// T: float, or double for the float64 FA_Tarboton (the only stage of that engine that reads the DEM)
+template <bool DINF, class T = float>
+__global__ void __launch_bounds__(256) flow_code_kernel(const T *__restrict__ dem, uint8_t *__restrict__ code,
                                                          float *__restrict__ rmaxArr, double *__restrict__ accum,
-                                                         int W, int H, float nodata, int ones, int tfilter) {
+                                                         int W, int H, T nodata, int ones, int tfilter) {
   const size_t n = (size_t)W * H;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -1935,13 +1936,21 @@ void fa_d8_tiles(const float *d_dem, double *d_accum, int w, int h, float nodata
 }
 }  // namespace
 
-// FA_D8 / FA_Tarboton fused (reference methods/flow_accumulation.hpp:27,16): no 36 B/cell props
-void fa_fused_dev(const float *d_dem, double *d_accum, int w, int h, float nodata, bool ones, bool dinf) {
+// FA_D8 / FA_Tarboton fused (reference methods/flow_accumulation.hpp:27,16): no 36 B/cell props.  T is the DEM's type;
+// only the code pass (flow_code_kernel) reads the DEM, everything after it works on the codes.  The D8 engines exist for
+// T = float only (the float64 FA_D8 runs on order-preserving float keys, f64.cu).
+template <class T>
+static void fa_fused(const T *d_dem, double *d_accum, int w, int h, T nodata, bool ones, bool dinf) {
+  constexpr bool F32 = sizeof(T) == 4;
   Ctx &c = ctx();
   const size_t n = (size_t)w * h;
-  if (!dinf && ones && c.params.accum_packed && fa_tile_slots(w, h) < INT32_MAX) {
-    fa_d8_tiles(d_dem, d_accum, w, h, nodata);  // unit-weight D8: tile by tile (see above)
-    return;
+  if constexpr (F32) {
+    if (!dinf && ones && c.params.accum_packed && fa_tile_slots(w, h) < INT32_MAX) {
+      fa_d8_tiles(d_dem, d_accum, w, h, nodata);  // unit-weight D8: tile by tile (see above)
+      return;
+    }
+  } else if (!dinf) {
+    fail("FA_D8 on doubles runs on float keys (fa_d8_f64_dev)");
   }
   DevBuf<uint8_t> code(n);
   DevBuf<float> rmax;
@@ -1955,7 +1964,7 @@ void fa_fused_dev(const float *d_dem, double *d_accum, int w, int h, float nodat
     rmax.alloc(n);
     const unsigned blocks = (unsigned)((n + 255) / 256);
     unsigned long long *word = reinterpret_cast<unsigned long long *>(d_accum);
-    flow_code_kernel<true><<<blocks, 256, 0, c.stream>>>(d_dem, code.p, rmax.p, d_accum, w, h, nodata, 1, (int)c.params.flowmet_tarboton_filter);
+    flow_code_kernel<true, T><<<blocks, 256, 0, c.stream>>>(d_dem, code.p, rmax.p, d_accum, w, h, nodata, 1, (int)c.params.flowmet_tarboton_filter);
     have_codes = true;
     DevBuf<DinfShare> share(1);
     RDB_CK(cudaMemsetAsync(share.p, 0, sizeof(DinfShare), c.stream));
@@ -2007,12 +2016,14 @@ void fa_fused_dev(const float *d_dem, double *d_accum, int w, int h, float nodat
   if (have_codes) {
     // flow codes, rmax and the unit weights are in place already
   } else if (dinf)
-    flow_code_kernel<true><<<blocks, 256, 0, c.stream>>>(d_dem, code.p, rmax.p, d_accum, w, h, nodata, ones ? 1 : 0, (int)c.params.flowmet_tarboton_filter);
-  else if ((w & 3) == 0 && ((uintptr_t)d_dem & 15) == 0 && ((uintptr_t)d_accum & 15) == 0) {
-    dim3 blk(256), grd((w / 4 + 255) / 256, h < 8192 ? h : 8192);
-    flow_code_d8_x4_kernel<<<grd, blk, 0, c.stream>>>(d_dem, code.p, d_accum, w, h, nodata, ones ? 1 : 0);
-  } else
-    flow_code_kernel<false><<<blocks, 256, 0, c.stream>>>(d_dem, code.p, nullptr, d_accum, w, h, nodata, ones ? 1 : 0, (int)c.params.flowmet_tarboton_filter);
+    flow_code_kernel<true, T><<<blocks, 256, 0, c.stream>>>(d_dem, code.p, rmax.p, d_accum, w, h, nodata, ones ? 1 : 0, (int)c.params.flowmet_tarboton_filter);
+  else if constexpr (F32) {
+    if ((w & 3) == 0 && ((uintptr_t)d_dem & 15) == 0 && ((uintptr_t)d_accum & 15) == 0) {
+      dim3 blk(256), grd((w / 4 + 255) / 256, h < 8192 ? h : 8192);
+      flow_code_d8_x4_kernel<<<grd, blk, 0, c.stream>>>(d_dem, code.p, d_accum, w, h, nodata, ones ? 1 : 0);
+    } else
+      flow_code_kernel<false><<<blocks, 256, 0, c.stream>>>(d_dem, code.p, nullptr, d_accum, w, h, nodata, ones ? 1 : 0, (int)c.params.flowmet_tarboton_filter);
+  }
   RDB_CK(cudaGetLastError());
   if ((w & 3) == 0) {
     dim3 blk(256), grd((w / 4 + 255) / 256, h < 8192 ? h : 8192);
@@ -2032,6 +2043,14 @@ void fa_fused_dev(const float *d_dem, double *d_accum, int w, int h, float nodat
   a.H = h;
   if (dinf) run_levels<1>(a, n);
   else run_walk<0, false, double>(a, n);
+}
+
+void fa_fused_dev(const float *d_dem, double *d_accum, int w, int h, float nodata, bool ones, bool dinf) {
+  fa_fused(d_dem, d_accum, w, h, nodata, ones, dinf);
+}
+// FA_Tarboton<double, double>: the same engine after a code pass on the doubles
+void fa_tarboton_f64_dev(const double *d_dem, double *d_accum, int w, int h, double nodata, bool ones) {
+  fa_fused(d_dem, d_accum, w, h, nodata, ones, true);
 }
 
 // FlowAccumulation(props, accum) (reference methods/flow_accumulation_generic.hpp:33-100)

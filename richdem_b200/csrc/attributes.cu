@@ -86,11 +86,13 @@ __device__ __forceinline__ double attribute(const Nbhd &t, const CellLen &lx, co
   return __dmul_rn(__ddiv_rn(__dmul_rn(2.0, num), den), 100.0);
 }
 
-template <int ATTR>
-__global__ void __launch_bounds__(kTW) terrain_attribute_kernel(const float *__restrict__ dem, float *__restrict__ out, int W, int H,
-                                                                float nodata_in, float nodata_out, float zscale, CellLen lx,
+// T: float, or double for rdb200_terrain_attribute_f64 (the reference reads T into its double neighbourhood,
+// terrain_attributes.hpp:172-190; only the window and the NoData test change type, the window to 18.7 KB)
+template <int ATTR, class T>
+__global__ void __launch_bounds__(kTW) terrain_attribute_kernel(const T *__restrict__ dem, float *__restrict__ out, int W, int H,
+                                                                T nodata_in, float nodata_out, float zscale, CellLen lx,
                                                                 CellLen ly) {
-  __shared__ float s[kTH + 2][kTW + 2];
+  __shared__ T s[kTH + 2][kTW + 2];
   const int x0 = blockIdx.x * kTW, y0 = blockIdx.y * kTH;
   // window load: cells outside the raster are marked by a flag row/column test at use, their slot is never read
   for (int r = 0; r < kTH + 2; r++) {
@@ -110,7 +112,7 @@ __global__ void __launch_bounds__(kTW) terrain_attribute_kernel(const float *__r
   for (int r = 1; r <= kTH; r++) {
     const int y = y0 + r - 1;
     if (y >= H) break;
-    const float ef = s[r][cx];
+    const T ef = s[r][cx];
     float o;
     if (ef == nodata_in) {  // terrain_attributes.hpp:349-350
       o = nodata_out;
@@ -118,9 +120,9 @@ __global__ void __launch_bounds__(kTW) terrain_attribute_kernel(const float *__r
       const bool has_u = y > 0, has_d = y + 1 < H;
       // neighbours outside the raster or NoData take the centre's value (:172-181)
       auto pick = [&](bool in, int rr, int cc) -> double {
-        float v = ef;
+        T v = ef;
         if (in) {
-          const float nv = s[rr][cc];
+          const T nv = s[rr][cc];
           if (nv != nodata_in) v = nv;
         }
         return __dmul_rn((double)v, zs);
@@ -141,8 +143,8 @@ __global__ void __launch_bounds__(kTW) terrain_attribute_kernel(const float *__r
   }
 }
 
-template <int ATTR>
-void launch(const float *d_dem, float *d_out, int w, int h, float nodata_in, float nodata_out, float zscale, double cell_x, double cell_y) {
+template <int ATTR, class T>
+void launch(const T *d_dem, float *d_out, int w, int h, T nodata_in, float nodata_out, float zscale, double cell_x, double cell_y) {
   Ctx &c = ctx();
   auto cell = [](double len) {
     int e = 0;
@@ -153,14 +155,14 @@ void launch(const float *d_dem, float *d_out, int w, int h, float nodata_in, flo
   };
   const CellLen lx = cell(cell_x), ly = cell(cell_y);
   const dim3 grd((w + kTW - 1) / kTW, (h + kTH - 1) / kTH);
-  terrain_attribute_kernel<ATTR><<<grd, kTW, 0, c.stream>>>(d_dem, d_out, w, h, nodata_in, nodata_out, zscale, lx, ly);
+  terrain_attribute_kernel<ATTR, T><<<grd, kTW, 0, c.stream>>>(d_dem, d_out, w, h, nodata_in, nodata_out, zscale, lx, ly);
   RDB_CK(cudaGetLastError());
+  count_launch();
 }
 
-}  // namespace
-
 // attribute: RDB200_TA_* (include/richdem_b200.h); cell_x / cell_y = |geotransform[1]|, |geotransform[5]|
-void terrain_attribute_dev(int attribute_id, const float *d_dem, float *d_out, int w, int h, float nodata_in, float nodata_out,
+template <class T>
+void terrain_attribute_any(int attribute_id, const T *d_dem, float *d_out, int w, int h, T nodata_in, float nodata_out,
                            float zscale, double cell_x, double cell_y) {
   if (!(cell_x > 0) || !(cell_y > 0)) fail("terrain attribute: cell lengths must be positive (got %g x %g)", cell_x, cell_y);
   switch (attribute_id) {
@@ -174,6 +176,17 @@ void terrain_attribute_dev(int attribute_id, const float *d_dem, float *d_out, i
     case RDB200_TA_PROFILE_CURVATURE: launch<RDB200_TA_PROFILE_CURVATURE>(d_dem, d_out, w, h, nodata_in, nodata_out, zscale, cell_x, cell_y); break;
     default: fail("unknown terrain attribute %d", attribute_id);
   }
+}
+
+}  // namespace
+
+void terrain_attribute_dev(int attribute_id, const float *d_dem, float *d_out, int w, int h, float nodata_in, float nodata_out,
+                           float zscale, double cell_x, double cell_y) {
+  terrain_attribute_any(attribute_id, d_dem, d_out, w, h, nodata_in, nodata_out, zscale, cell_x, cell_y);
+}
+void terrain_attribute_f64_dev(int attribute_id, const double *d_dem, float *d_out, int w, int h, double nodata_in,
+                               float nodata_out, float zscale, double cell_x, double cell_y) {
+  terrain_attribute_any(attribute_id, d_dem, d_out, w, h, nodata_in, nodata_out, zscale, cell_x, cell_y);
 }
 
 }  // namespace rdb

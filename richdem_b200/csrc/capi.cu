@@ -706,6 +706,114 @@ int rdb200_fa_d4_f64_f64(const double *dem, double *accum, int32_t w, int32_t h,
   CAPI_END
 }
 
+// ---- float64 D-infinity, MFD and terrain attributes: the float kernels' double instantiations (no keys: these stages do
+// arithmetic on the elevations, DESIGN §0.2).  Argument order and checks as the float entry points above.
+
+// reference flowmet/*.hpp with E = double; method numbered as fm_dispatch_dev
+static int fm_f64_host(const double *dem, float *props, int32_t w, int32_t h, double nodata, int method, double xparam = 0) {
+  CAPI_TRY
+  if (!dem || !props) fail("flow metric: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n);
+  DevBuf<float> p(9 * n);
+  h2d(d.p, dem, n);
+  fm_method_f64_dev(method, d.p, p.p, w, h, nodata, xparam);
+  d2h(props, p.p, 9 * n);
+  cs.done();
+  CAPI_END
+}
+int rdb200_fm_d8_f64(const double *dem, float *props, int32_t w, int32_t h, double nodata) {
+  return fm_f64_host(dem, props, w, h, nodata, 0);
+}
+int rdb200_fm_tarboton_f64(const double *dem, float *props, int32_t w, int32_t h, double nodata) {
+  return fm_f64_host(dem, props, w, h, nodata, 1);
+}
+int rdb200_fm_d4_f64(const double *dem, float *props, int32_t w, int32_t h, double nodata) {
+  return fm_f64_host(dem, props, w, h, nodata, 2);
+}
+int rdb200_fm_quinn_f64(const double *dem, float *props, int32_t w, int32_t h, double nodata) {
+  return fm_f64_host(dem, props, w, h, nodata, 3, 1.0);
+}
+int rdb200_fm_holmgren_f64(const double *dem, float *props, int32_t w, int32_t h, double nodata, double xparam) {
+  return fm_f64_host(dem, props, w, h, nodata, 3, xparam);
+}
+int rdb200_fm_freeman_f64(const double *dem, float *props, int32_t w, int32_t h, double nodata, double xparam) {
+  return fm_f64_host(dem, props, w, h, nodata, 4, xparam);
+}
+
+// methods/flow_accumulation.hpp:16-20 with E = double: FM_x on the doubles into device-side proportions + the generic
+// accumulation; methods 0 and 2 take the key route of FA_D8 / FA_D4 (accum holds the weights)
+static void fa_method_f64_dev(int method, const double *d_dem, double *d_accum, int w, int h, double nodata, double xparam) {
+  if (method == 0) {
+    fa_d8_f64_dev(d_dem, d_accum, w, h, nodata, false);
+  } else if (method == 2) {
+    fa_d4_f64_dev(d_dem, d_accum, w, h, nodata);
+  } else {
+    DevBuf<float> p(9 * (size_t)w * h);
+    fm_method_f64_dev(method, d_dem, p.p, w, h, nodata, xparam);
+    flow_accumulation_props_dev(p.p, d_accum, w, h);
+  }
+}
+static int fa_method_f64_host(int method, const double *dem, double *accum, int32_t w, int32_t h, double nodata, double xparam) {
+  CAPI_TRY
+  if (!dem || !accum) fail("flow accumulation: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n), a(n);
+  h2d(d.p, dem, n);
+  h2d(a.p, accum, n);
+  fa_method_f64_dev(method, d.p, a.p, w, h, nodata, xparam);
+  d2h(accum, a.p, n);
+  cs.done();
+  CAPI_END
+}
+int rdb200_fa_quinn_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata) {
+  return fa_method_f64_host(3, dem, accum, w, h, nodata, 1.0);
+}
+int rdb200_fa_holmgren_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata, double xparam) {
+  return fa_method_f64_host(3, dem, accum, w, h, nodata, xparam);
+}
+int rdb200_fa_freeman_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata, double xparam) {
+  return fa_method_f64_host(4, dem, accum, w, h, nodata, xparam);
+}
+
+// methods/flow_accumulation.hpp:16 (FA_Tarboton<double, double>): the fused D-infinity engine after a code pass on the
+// doubles; accum_is_ones as rdb200_fa_tarboton_f32_f64
+int rdb200_fa_tarboton_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata, int32_t ones) {
+  CAPI_TRY
+  if (!dem || !accum) fail("flow accumulation: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n), a(n);
+  h2d(d.p, dem, n);
+  if (!ones) h2d(a.p, accum, n);
+  fa_tarboton_f64_dev(d.p, a.p, w, h, nodata, ones != 0);
+  d2h(accum, a.p, n);
+  cs.done();
+  CAPI_END
+}
+
+// methods/terrain_attributes.hpp:370-538 with T = double: 8 B in + 4 B out per cell
+int rdb200_terrain_attribute_f64(int32_t attribute, const double *dem, float *out, int32_t w, int32_t h, double nodata_in,
+                                 float nodata_out, float zscale, double cell_x, double cell_y) {
+  CAPI_TRY
+  if (!dem || !out) fail("terrain attribute: null pointer");
+  check_dims(w, h);
+  CallScope cs((int64_t)w * h);
+  const size_t n = (size_t)w * h;
+  DevBuf<double> d(n);
+  DevBuf<float> o(n);
+  h2d(d.p, dem, n);
+  terrain_attribute_f64_dev(attribute, d.p, o.p, w, h, nodata_in, nodata_out, zscale, cell_x, cell_y);
+  d2h(out, o.p, n);
+  cs.done();
+  CAPI_END
+}
+
 // kappa itself: the float keys the entry points above run the float engines on, kappa(nodata) and which case ran
 int rdb200_f64_order_keys(const double *dem, float *keys, int32_t w, int32_t h, double nodata, float *nodata_key,
                           int32_t *ranked) {
@@ -863,6 +971,22 @@ int rdb200_dev_fa_d8_f64_f64(const double *d_dem, double *d_accum, int32_t w, in
 }
 int rdb200_dev_fa_d4_f64_f64(const double *d_dem, double *d_accum, int32_t w, int32_t h, double nodata) {
   DEV_ENTRY((int64_t)w * h, (check_dims(w, h), fa_d4_f64_dev(d_dem, d_accum, w, h, nodata)))
+}
+int rdb200_dev_fm_method_f64(int32_t method, const double *d_dem, float *d_props, int32_t w, int32_t h, double nodata,
+                             double xparam) {
+  DEV_ENTRY((int64_t)w * h, (check_dims(w, h), fm_method_f64_dev(method, d_dem, d_props, w, h, nodata, xparam)))
+}
+int rdb200_dev_fa_method_f64_f64(int32_t method, const double *d_dem, double *d_accum, int32_t w, int32_t h, double nodata,
+                                 double xparam) {
+  DEV_ENTRY((int64_t)w * h, (check_dims(w, h), fa_method_f64_dev(method, d_dem, d_accum, w, h, nodata, xparam)))
+}
+int rdb200_dev_fa_tarboton_f64_f64(const double *d_dem, double *d_accum, int32_t w, int32_t h, double nodata, int32_t ones) {
+  DEV_ENTRY((int64_t)w * h, (check_dims(w, h), fa_tarboton_f64_dev(d_dem, d_accum, w, h, nodata, ones != 0)))
+}
+int rdb200_dev_terrain_attribute_f64(int32_t attribute, const double *d_dem, float *d_out, int32_t w, int32_t h,
+                                     double nodata_in, float nodata_out, float zscale, double cell_x, double cell_y) {
+  DEV_ENTRY((int64_t)w * h, (check_dims(w, h), terrain_attribute_f64_dev(attribute, d_dem, d_out, w, h, nodata_in, nodata_out,
+                                                                        zscale, cell_x, cell_y)))
 }
 int rdb200_dev_f64_order_keys(const double *d_dem, float *d_keys, int32_t w, int32_t h, double nodata, float *nodata_key,
                               int32_t *ranked) {

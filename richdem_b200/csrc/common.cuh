@@ -226,5 +226,11 @@ void pit_mask_f64_dev(const double *d_z, uint8_t *d_mask, int w, int h, double n
 bool has_depressions_f64_dev(const double *d_z, int w, int h, bool topo4);
 void resolve_flats_f64_dev(double *d_z, int w, int h, double nodata);
 void fa_d8_f64_dev(const double *d_z, double *d_accum, int w, int h, double nodata, bool ones);
+// D-infinity, MFD and terrain attributes on doubles: the float kernels' double instantiations (flowdirs.cu, accum.cu,
+// attributes.cu), no keys -- these stages do arithmetic on the elevations
+void fm_method_f64_dev(int method, const double *d_dem, float *d_props, int w, int h, double nodata, double xparam);
+void fa_tarboton_f64_dev(const double *d_dem, double *d_accum, int w, int h, double nodata, bool ones);
+void terrain_attribute_f64_dev(int attribute_id, const double *d_dem, float *d_out, int w, int h, double nodata_in,
+                               float nodata_out, float zscale, double cell_x, double cell_y);
 
 }  // namespace rdb

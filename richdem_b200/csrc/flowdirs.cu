@@ -126,9 +126,10 @@ __global__ void __launch_bounds__(256) d8_flowdirs_rolling_kernel(const float *_
 // MODE: 0 FM_D8, 1 FM_Tarboton, 2 FM_D4, 3 FM_Holmgren (FM_Quinn = exponent 1), 4 FM_Freeman
 enum : int { FM_MODE_D8 = 0, FM_MODE_DINF = 1, FM_MODE_D4 = 2, FM_MODE_HOLMGREN = 3, FM_MODE_FREEMAN = 4 };
 
-template <int MODE>
-__global__ void __launch_bounds__(256) fm_props_kernel(const float *__restrict__ dem, float *__restrict__ props,
-                                                        int W, int H, float nodata, double xparam, int tfilter) {
+// T: float, or double for the rdb200_fm_*_f64 entry points (8 B in per cell instead of 4)
+template <int MODE, class T>
+__global__ void __launch_bounds__(256) fm_props_kernel(const T *__restrict__ dem, float *__restrict__ props,
+                                                        int W, int H, T nodata, double xparam, int tfilter) {
   constexpr bool DINF = MODE == FM_MODE_DINF;
   __shared__ __align__(16) float s[256 * 9];
   const size_t n = (size_t)W * H;
@@ -229,11 +230,11 @@ void d8_flow_directions_f64_dev(const double *d_dem, uint8_t *d_dirs, int w, int
   count_launch();
 }
 
-template <int MODE>
-static void fm_launch(const float *d_dem, float *d_props, int w, int h, float nodata, double xparam) {
+template <int MODE, class T>
+static void fm_launch(const T *d_dem, float *d_props, int w, int h, T nodata, double xparam) {
   Ctx &c = ctx();
   const size_t n = (size_t)w * h;
-  fm_props_kernel<MODE><<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(d_dem, d_props, w, h, nodata, xparam,
+  fm_props_kernel<MODE, T><<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(d_dem, d_props, w, h, nodata, xparam,
                                                                            (int)c.params.flowmet_tarboton_filter);
   RDB_CK(cudaGetLastError());
   count_launch();
@@ -253,6 +254,19 @@ void fm_holmgren_dev(const float *d_dem, float *d_props, int w, int h, float nod
 }
 void fm_freeman_dev(const float *d_dem, float *d_props, int w, int h, float nodata, double xparam) {
   fm_launch<FM_MODE_FREEMAN>(d_dem, d_props, w, h, nodata, xparam);
+}
+
+// the same five metrics on doubles (reference templates with E = double), by the C ABI's method number:
+// 0 FM_D8, 1 FM_Tarboton, 2 FM_D4, 3 FM_Holmgren (FM_Quinn = exponent 1), 4 FM_Freeman
+void fm_method_f64_dev(int method, const double *d_dem, float *d_props, int w, int h, double nodata, double xparam) {
+  switch (method) {
+    case 0: fm_launch<FM_MODE_D8>(d_dem, d_props, w, h, nodata, 0.0); break;
+    case 1: fm_launch<FM_MODE_DINF>(d_dem, d_props, w, h, nodata, 0.0); break;
+    case 2: fm_launch<FM_MODE_D4>(d_dem, d_props, w, h, nodata, 0.0); break;
+    case 3: fm_launch<FM_MODE_HOLMGREN>(d_dem, d_props, w, h, nodata, xparam); break;
+    case 4: fm_launch<FM_MODE_FREEMAN>(d_dem, d_props, w, h, nodata, xparam); break;
+    default: fail("unknown flow metric %d", method);
+  }
 }
 
 }  // namespace rdb

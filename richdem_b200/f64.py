@@ -1,10 +1,13 @@
 """float64 elevations on the GPU: ``FillDepressions``, ``PitMask``, ``HasDepressions``, ``ResolveFlats``,
-``FlowAccumulation`` (D8 / OCallaghanD8 / D4 / OCallaghanD4) and ``FlowDirectionsD8`` for C-contiguous float64
-``rdarray``s, with the arguments, checks and messages of the float32 functions in :mod:`richdem_b200`.
+``FlowAccumulation`` (D8 / OCallaghanD8 / D4 / OCallaghanD4), ``FlowDirectionsD8``, ``FlowProportions`` and
+``TerrainAttribute`` for C-contiguous float64 ``rdarray``s, with the arguments, checks and messages of the float32
+functions in :mod:`richdem_b200`.
 
-Each call gives what the reference's ``double`` templates give (the fill's zero sign aside, as for float32): the float
-engines run on an order-preserving float key of every value, so two levels one double ulp apart stay apart.  Casting to
-float32 first does not do that.  See DESIGN §0.
+Each call gives what the reference's ``double`` templates give (the fill's zero sign aside, as for float32), within the
+float32 path's tolerances.  The stages that only compare elevations run the float engines on an order-preserving float
+key of every value, so two levels one double ulp apart stay apart (DESIGN §0.1).  ``FlowProportions`` and
+``TerrainAttribute`` do arithmetic on the elevations and run double instantiations of the float kernels (DESIGN §0.2).
+Casting to float32 first gives neither answer.
 """
 from __future__ import annotations
 
@@ -15,7 +18,7 @@ import numpy as np
 
 from . import _lib
 from . import (_D4_METHODS, _D8_METHODS, _DINF_METHODS, _EXPONENT_METHODS, _OUT_OF_SCOPE_METHODS, _accum_array,
-               _add_analysis, rdarray)
+               _add_analysis, _terrain_attrib_id, rd3array, rdarray)
 
 
 def _dem_f64(dem: rdarray, what: str) -> np.ndarray:
@@ -109,7 +112,10 @@ def ResolveFlats(dem: rdarray, in_place: bool = False) -> Optional[rdarray]:
 def FlowAccumulation(dem: rdarray, method: Optional[str] = None, exponent: Optional[float] = None,
                      weights: Optional[rdarray] = None, in_place: bool = False) -> rdarray:
     """FA_D8<double, double> (``D8`` / ``OCallaghanD8``) and FA_D4<double, double> (``D4`` / ``OCallaghanD4``).  The
-    other methods do arithmetic on elevation differences and are not available for float64 rasters."""
+    other methods are refused here.  Float64 D-infinity, Quinn, Holmgren and Freeman accumulation is available through
+    ``richdem_b200.FlowAccumFromProps(f64.FlowProportions(dem, method, exponent))``, through the C ABI
+    (``rdb200_fa_{tarboton,quinn,holmgren,freeman}_f64_f64``) and through the C++ specialisations of
+    ``include/richdem_b200.hpp`` under ``RICHDEM_B200_F64`` (and so the reference's own Python package built on them)."""
     if type(dem) is not rdarray:
         raise Exception("A richdem.rdarray or numpy.ndarray is required!")
     accum, ones = _accum_array(dem, weights, in_place, dem.shape)
@@ -145,6 +151,60 @@ def FlowDirectionsD8(dem: rdarray) -> rdarray:
     _lib.check(_lib.lib().rdb200_d8_flow_directions_f64(_lib.ptr(d), _lib.ptr(out), w, h, _nodata_f64(dem)))
     out.no_data = 255
     return out
+
+
+def FlowProportions(dem: rdarray, method: Optional[str] = None, exponent: Optional[float] = None) -> rd3array:
+    """FM_x<double> (reference FlowProportions, :650-732): (H, W, 9) float32 proportions of a float64 raster, laid out
+    as :func:`richdem_b200.FlowProportions` lays them out."""
+    if type(dem) is not rdarray:
+        raise Exception("A richdem.rdarray or numpy.ndarray is required!")
+    fprops = rd3array(np.empty(shape=dem.shape + (9,), dtype="float32"), meta_obj=dem, no_data=-2)
+    _add_analysis(fprops, f"FlowProportions(dem, method={method}, exponent={exponent})")
+    d = _dem_f64(dem, "FlowProportions")
+    h, w = d.shape
+    L = _lib.lib()
+    nd = _nodata_f64(dem)
+    if method in _D8_METHODS:
+        _lib.check(L.rdb200_fm_d8_f64(_lib.ptr(d), _lib.ptr(fprops), w, h, nd))
+    elif method in _DINF_METHODS:
+        _lib.check(L.rdb200_fm_tarboton_f64(_lib.ptr(d), _lib.ptr(fprops), w, h, nd))
+    elif method in _D4_METHODS:
+        _lib.check(L.rdb200_fm_d4_f64(_lib.ptr(d), _lib.ptr(fprops), w, h, nd))
+    elif method == "Quinn":
+        _lib.check(L.rdb200_fm_quinn_f64(_lib.ptr(d), _lib.ptr(fprops), w, h, nd))
+    elif method in _EXPONENT_METHODS:
+        if exponent is None:
+            raise Exception('FlowProportions method "' + method + '" requires an exponent!')
+        fn = L.rdb200_fm_freeman_f64 if method == "Freeman" else L.rdb200_fm_holmgren_f64
+        _lib.check(fn(_lib.ptr(d), _lib.ptr(fprops), w, h, nd, float(exponent)))
+    elif method in _OUT_OF_SCOPE_METHODS:
+        raise Exception(f'FlowProportions method "{method}" is outside the GPU hot path '
+                        "(random-walk metric; use the reference CPU implementation)")
+    else:
+        raise Exception("Invalid FlowProportions method. Valid methods are: " +
+                        ", ".join(_DINF_METHODS + ("Quinn",) + _D8_METHODS + _D4_METHODS + _EXPONENT_METHODS +
+                                  _OUT_OF_SCOPE_METHODS))
+    fprops.no_data = -2
+    return fprops
+
+
+def TerrainAttribute(dem: rdarray, attrib: str, zscale: float = 1.0) -> rdarray:
+    """TA_x<double> (reference TerrainAttribute, :735-794) of a float64 raster: float32 result with no_data -9999, cell
+    lengths from the geotransform (1 x 1 when there is none), as :func:`richdem_b200.TerrainAttribute`."""
+    if type(dem) is not rdarray:
+        raise Exception("A richdem.rdarray or numpy.ndarray is required!")
+    attrib_id = _terrain_attrib_id(attrib)
+    d = _dem_f64(dem, "TerrainAttribute")
+    h, w = d.shape
+    gt = dem.geotransform
+    if gt is None:
+        print("Warning! No geotransform defined. Choosing a standard one! (Top left cell's top let corner at <0,0>; cells are 1x1.)")
+        gt = [0, 1, 0, 0, 0, -1]
+    result = rdarray(np.zeros((h, w), np.float32), meta_obj=dem, no_data=-9999)
+    _add_analysis(result, f"TerrainAttribute(dem, attrib={attrib}, zscale={zscale})")
+    _lib.check(_lib.lib().rdb200_terrain_attribute_f64(attrib_id, _lib.ptr(d), _lib.ptr(result), w, h, _nodata_f64(dem),
+                                                        -9999.0, float(zscale), abs(float(gt[1])), abs(float(gt[5]))))
+    return result
 
 
 def OrderKeys(dem: np.ndarray, no_data: float = -9999.0):
