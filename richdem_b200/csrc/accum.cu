@@ -15,6 +15,7 @@
 
 #include <cmath>
 #include <cooperative_groups.h>
+#include <memory>
 namespace cg = cooperative_groups;
 
 namespace rdb {
@@ -2860,40 +2861,24 @@ void mgpu_d8_flow_accum_band(const rdb200_comm *comm, const uint8_t *d_dirs, int
   RDB_CK(cudaStreamSynchronize(c.stream));
 }
 
-void capi_set_error(const char *msg);
-
 }  // namespace rdb
 
 struct rdb200_facc_state {
   rdb::FaccState st;
 };
 
-#define FACC_TRY try {
-#define FACC_END                        \
-  }                                     \
-  catch (const std::exception &e) {     \
-    rdb::capi_set_error(e.what());      \
-    return 1;                           \
-  }                                     \
-  return 0;
-
 extern "C" {
 
 int rdb200_dev_facc_begin_method(rdb200_facc_state **state, const float *d_dem, double *d_accum_inout, int32_t width,
                                  int32_t height, float nodata, int32_t ghost_top, int32_t ghost_bottom, int32_t method,
                                  double xparam, int32_t accum_is_ones) {
-  FACC_TRY
-  rdb::ensure_init();
-  if (!state || !d_dem || !d_accum_inout) rdb::fail("facc_begin: null pointer");
-  auto *s = new rdb200_facc_state();
-  try {
+  return rdb::capi_call([&] {
+    rdb::ensure_init();
+    if (!state || !d_dem || !d_accum_inout) rdb::fail("facc_begin: null pointer");
+    auto s = std::make_unique<rdb200_facc_state>();
     s->st.begin(d_dem, d_accum_inout, width, height, nodata, ghost_top, ghost_bottom, method, xparam, accum_is_ones != 0);
-  } catch (...) {
-    delete s;
-    throw;
-  }
-  *state = s;
-  FACC_END
+    *state = s.release();
+  });
 }
 
 int rdb200_dev_facc_begin(rdb200_facc_state **state, const float *d_dem, double *d_accum_inout, int32_t width,
@@ -2904,52 +2889,52 @@ int rdb200_dev_facc_begin(rdb200_facc_state **state, const float *d_dem, double 
 }
 
 int rdb200_dev_facc_get_edge_codes(rdb200_facc_state *state, int32_t which, uint8_t *d_code_row, float *d_rmax_row) {
-  FACC_TRY
-  state->st.get_edge_codes(which, d_code_row, d_rmax_row);
-  RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
-  FACC_END
+  return rdb::capi_call([&] {
+    state->st.get_edge_codes(which, d_code_row, d_rmax_row);
+    RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
+  });
 }
 
 int rdb200_dev_facc_set_ghost_codes(rdb200_facc_state *state, int32_t which, const uint8_t *d_code_row,
                                     const float *d_rmax_row) {
-  FACC_TRY
-  state->st.set_ghost_codes(which, d_code_row, d_rmax_row);
-  RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
-  FACC_END
+  return rdb::capi_call([&] {
+    state->st.set_ghost_codes(which, d_code_row, d_rmax_row);
+    RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
+  });
 }
 
 int rdb200_dev_facc_run(rdb200_facc_state *state, int32_t *sent_top, int32_t *sent_bottom) {
-  FACC_TRY
-  state->st.collect_frontier();
-  int a = 0, b = 0;
-  state->st.run(&a, &b);
-  if (sent_top) *sent_top = a;
-  if (sent_bottom) *sent_bottom = b;
-  FACC_END
+  return rdb::capi_call([&] {
+    state->st.collect_frontier();
+    int a = 0, b = 0;
+    state->st.run(&a, &b);
+    if (sent_top) *sent_top = a;
+    if (sent_bottom) *sent_bottom = b;
+  });
 }
 
 int rdb200_dev_facc_take_outflow(rdb200_facc_state *state, int32_t which, double *d_sum_row, int32_t *d_cnt_row) {
-  FACC_TRY
-  state->st.take_outflow(which, d_sum_row, d_cnt_row);
-  RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
-  FACC_END
+  return rdb::capi_call([&] {
+    state->st.take_outflow(which, d_sum_row, d_cnt_row);
+    RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
+  });
 }
 
 int rdb200_dev_facc_apply_inflow(rdb200_facc_state *state, int32_t which, const double *d_sum_row,
                                  const int32_t *d_cnt_row) {
-  FACC_TRY
-  state->st.apply_inflow(which, d_sum_row, d_cnt_row);
-  RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
-  FACC_END
+  return rdb::capi_call([&] {
+    state->st.apply_inflow(which, d_sum_row, d_cnt_row);
+    RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
+  });
 }
 
 int rdb200_dev_facc_finish(rdb200_facc_state *state) {
-  FACC_TRY
-  if (state) {
-    RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
-    delete state;
-  }
-  FACC_END
+  return rdb::capi_call([&] {
+    if (state) {
+      RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
+      delete state;
+    }
+  });
 }
 
 }  // extern "C"

@@ -10,6 +10,7 @@
 #include "common.cuh"
 
 #include <dlfcn.h>
+#include <memory>
 
 namespace rdb {
 
@@ -144,73 +145,57 @@ void exchange_band_rows(const rdb200_comm *comm, void *d_band, size_t elem, int 
   comm_exchange(comm, b + (size_t)gt * row, b, b + (size_t)(hloc - 1 - gb) * row, b + (size_t)(hloc - 1) * row, row);
 }
 
-void capi_set_error(const char *msg);
-
 }  // namespace rdb
-
-#define COMM_TRY try {
-#define COMM_END                      \
-  }                                   \
-  catch (const std::exception &e) {   \
-    rdb::capi_set_error(e.what());    \
-    return 1;                         \
-  }                                   \
-  return 0;
 
 extern "C" {
 
 int rdb200_nccl_unique_id(uint8_t *out128) {
-  COMM_TRY
-  if (!out128) rdb::fail("nccl_unique_id: null pointer");
-  rdb::NcclUniqueId id;
-  rdb::nccl_ck(rdb::nccl().GetUniqueId(&id), "get unique id");
-  memcpy(out128, id.internal, 128);
-  COMM_END
+  return rdb::capi_call([&] {
+    if (!out128) rdb::fail("nccl_unique_id: null pointer");
+    rdb::NcclUniqueId id;
+    rdb::nccl_ck(rdb::nccl().GetUniqueId(&id), "get unique id");
+    memcpy(out128, id.internal, 128);
+  });
 }
 
 int rdb200_comm_create_nccl(rdb200_comm **out, int32_t rank, int32_t world, const uint8_t *id128) {
-  COMM_TRY
-  rdb::ensure_init();  // the communicator binds to this process's device
-  if (!out || !id128 || world < 1 || rank < 0 || rank >= world) rdb::fail("comm_create_nccl: bad arguments");
-  auto *c = new rdb200_comm();
-  c->rank = rank;
-  c->world = world;
-  if (world > 1) {
-    rdb::NcclUniqueId id;
-    memcpy(id.internal, id128, 128);
-    try {
+  return rdb::capi_call([&] {
+    rdb::ensure_init();  // the communicator binds to this process's device
+    if (!out || !id128 || world < 1 || rank < 0 || rank >= world) rdb::fail("comm_create_nccl: bad arguments");
+    auto c = std::make_unique<rdb200_comm>();
+    c->rank = rank;
+    c->world = world;
+    if (world > 1) {
+      rdb::NcclUniqueId id;
+      memcpy(id.internal, id128, 128);
       rdb::nccl_ck(rdb::nccl().CommInitRank(&c->nccl, world, id, rank), "communicator init");
-    } catch (...) {
-      delete c;
-      throw;
     }
-  }
-  *out = c;
-  COMM_END
+    *out = c.release();
+  });
 }
 
 int rdb200_comm_create_callbacks(rdb200_comm **out, int32_t rank, int32_t world, void *user, rdb200_exchange_fn exchange,
                                  rdb200_allreduce_fn allreduce) {
-  COMM_TRY
-  if (!out || world < 1 || rank < 0 || rank >= world || (world > 1 && (!exchange || !allreduce)))
-    rdb::fail("comm_create_callbacks: bad arguments");
-  auto *c = new rdb200_comm();
-  c->rank = rank;
-  c->world = world;
-  c->user = user;
-  c->exchange = exchange;
-  c->allreduce = allreduce;
-  *out = c;
-  COMM_END
+  return rdb::capi_call([&] {
+    if (!out || world < 1 || rank < 0 || rank >= world || (world > 1 && (!exchange || !allreduce)))
+      rdb::fail("comm_create_callbacks: bad arguments");
+    auto *c = new rdb200_comm();
+    c->rank = rank;
+    c->world = world;
+    c->user = user;
+    c->exchange = exchange;
+    c->allreduce = allreduce;
+    *out = c;
+  });
 }
 
 int rdb200_comm_destroy(rdb200_comm *c) {
-  COMM_TRY
-  if (c) {
-    if (c->nccl) rdb::nccl().CommDestroy(c->nccl);
-    delete c;
-  }
-  COMM_END
+  return rdb::capi_call([&] {
+    if (c) {
+      if (c->nccl) rdb::nccl().CommDestroy(c->nccl);
+      delete c;
+    }
+  });
 }
 
 }  // extern "C"

@@ -39,6 +39,23 @@ struct Error : std::runtime_error {
       ::rdb::fail("%s failed at %s:%d: %s", #expr, __FILE__, __LINE__, cudaGetErrorString(_e)); \
   } while (0)
 
+void capi_set_error(const char *msg);  // the text rdb200_last_error() returns
+
+// The error boundary of every extern "C" entry point: nothing thrown may cross the C ABI.  Runs body and returns 0, or 1
+// with what was thrown as the last error.
+template <class F>
+int capi_call(F &&body) {
+  try {
+    body();
+    return 0;
+  } catch (const std::exception &e) {
+    capi_set_error(e.what());
+  } catch (...) {
+    capi_set_error("unknown C++ exception");
+  }
+  return 1;
+}
+
 // ---- D8 tables (reference include/richdem/common/constants.hpp:44-45,65) ----------------
 //   2 3 4
 //   1 0 5

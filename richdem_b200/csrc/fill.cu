@@ -28,6 +28,7 @@
 #include "common.cuh"
 
 #include <chrono>
+#include <memory>
 
 namespace rdb {
 
@@ -2084,141 +2085,118 @@ int mgpu_relax_band(const rdb200_comm *comm, rdb200_fill_state *state, int gt, i
 }
 }  // namespace rdb
 
-namespace rdb {
-void capi_set_error(const char *msg);
-}  // namespace rdb
-
-#define RDB_CAPI_TRY try {
-#define RDB_CAPI_END                 \
-  }                                  \
-  catch (const std::exception &e) {  \
-    rdb::capi_set_error(e.what());   \
-    return 1;                        \
-  }                                  \
-  return 0;
-
 extern "C" {
 
 int rdb200_dev_fill_begin(rdb200_fill_state **state, const float *d_dem, int32_t width, int32_t height) {
-  RDB_CAPI_TRY
-  rdb::ensure_init();
-  if (!state) rdb::fail("fill_begin: null state pointer");
-  if (width < 3 || height < 3) rdb::fail("fill_begin: band must be at least 3x3");
-  auto *s = new rdb200_fill_state();
-  try {
+  return rdb::capi_call([&] {
+    rdb::ensure_init();
+    if (!state) rdb::fail("fill_begin: null state pointer");
+    if (width < 3 || height < 3) rdb::fail("fill_begin: band must be at least 3x3");
+    auto s = std::make_unique<rdb200_fill_state>();
     s->st.begin(d_dem, width, height);
-  } catch (...) {
-    delete s;
-    throw;
-  }
-  *state = s;
-  RDB_CAPI_END
+    *state = s.release();
+  });
 }
 
 int rdb200_dev_fill_begin_lifted(rdb200_fill_state **state, const float *d_dem, int32_t width, int32_t height,
                                  const float *d_coarse, int32_t coarse_width, int32_t pool, int32_t row_offset) {
-  RDB_CAPI_TRY
-  rdb::ensure_init();
-  if (!state) rdb::fail("fill_begin_lifted: null state pointer");
-  if (width < 3 || height < 3) rdb::fail("fill_begin_lifted: band must be at least 3x3");
-  if (!d_coarse || pool < 2 || coarse_width < (width + pool - 1) / pool || row_offset < 0)
-    rdb::fail("fill_begin_lifted: bad coarse raster (pool %d, coarse_width %d, row_offset %d)", pool, coarse_width, row_offset);
-  auto *s = new rdb200_fill_state();
-  try {
+  return rdb::capi_call([&] {
+    rdb::ensure_init();
+    if (!state) rdb::fail("fill_begin_lifted: null state pointer");
+    if (width < 3 || height < 3) rdb::fail("fill_begin_lifted: band must be at least 3x3");
+    if (!d_coarse || pool < 2 || coarse_width < (width + pool - 1) / pool || row_offset < 0)
+      rdb::fail("fill_begin_lifted: bad coarse raster (pool %d, coarse_width %d, row_offset %d)", pool, coarse_width, row_offset);
+    auto s = std::make_unique<rdb200_fill_state>();
     s->st.begin(d_dem, width, height, d_coarse, coarse_width, pool, row_offset);
-  } catch (...) {
-    delete s;
-    throw;
-  }
-  *state = s;
-  RDB_CAPI_END
+    *state = s.release();
+  });
 }
 
 int rdb200_dev_maxpool_rows_f32(const float *d_src, int32_t width, int32_t height, int32_t row_offset, int32_t pool,
                                 float *d_coarse, int32_t coarse_width, int32_t coarse_height) {
-  RDB_CAPI_TRY
-  rdb::ensure_init();
-  if (width < 1 || height < 1 || pool < 2 || row_offset < 0 || coarse_width < (width + pool - 1) / pool ||
-      coarse_height < (row_offset + height + pool - 1) / pool)
-    rdb::fail("maxpool_rows: bad geometry");
-  rdb::Ctx &c = rdb::ctx();
-  dim3 blk(256), grd((unsigned)((coarse_width + 255) / 256), (unsigned)(height / pool + 2 < 4096 ? height / pool + 2 : 4096));
-  rdb::fill_maxpool_rows(d_src, width, height, row_offset, d_coarse, coarse_width, coarse_height, pool, grd, blk);
-  RDB_CK(cudaStreamSynchronize(c.stream));
-  RDB_CAPI_END
+  return rdb::capi_call([&] {
+    rdb::ensure_init();
+    if (width < 1 || height < 1 || pool < 2 || row_offset < 0 || coarse_width < (width + pool - 1) / pool ||
+        coarse_height < (row_offset + height + pool - 1) / pool)
+      rdb::fail("maxpool_rows: bad geometry");
+    rdb::Ctx &c = rdb::ctx();
+    dim3 blk(256), grd((unsigned)((coarse_width + 255) / 256), (unsigned)(height / pool + 2 < 4096 ? height / pool + 2 : 4096));
+    rdb::fill_maxpool_rows(d_src, width, height, row_offset, d_coarse, coarse_width, coarse_height, pool, grd, blk);
+    RDB_CK(cudaStreamSynchronize(c.stream));
+  });
 }
 
 int rdb200_dev_fill_relax_from_f32(const float *d_dem, float *d_w_inout, int32_t width, int32_t height) {
-  RDB_CAPI_TRY
-  rdb::ensure_init();
-  if (width < 1 || height < 1) rdb::fail("fill_relax_from: raster dimensions must be positive");
-  rdb::fill_relax_from_dev(d_dem, d_w_inout, width, height);
-  RDB_CAPI_END
+  return rdb::capi_call([&] {
+    rdb::ensure_init();
+    if (width < 1 || height < 1) rdb::fail("fill_relax_from: raster dimensions must be positive");
+    rdb::fill_relax_from_dev(d_dem, d_w_inout, width, height);
+  });
 }
 
 int rdb200_dev_fill_blockmax(rdb200_fill_state *state, float *d_blockmax, int32_t coarse_width, int32_t coarse_height, int32_t pool,
                              int32_t row_offset, int32_t skip_top, int32_t skip_bottom) {
-  RDB_CAPI_TRY
-  if (!state) rdb::fail("fill_blockmax: null state");
-  rdb::FillState &st = state->st;
-  if (pool < 2 || row_offset < 0 || skip_top < 0 || skip_bottom < 0 || skip_top + skip_bottom >= st.H ||
-      coarse_width < (st.W + pool - 1) / pool || coarse_height < (row_offset + st.H - skip_bottom + pool - 1) / pool)
-    rdb::fail("fill_blockmax: bad geometry");
-  st.blockmax_into(d_blockmax, coarse_width, coarse_height, pool, row_offset, skip_top, st.H - skip_bottom);
-  RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
-  RDB_CAPI_END
+  return rdb::capi_call([&] {
+    if (!state) rdb::fail("fill_blockmax: null state");
+    rdb::FillState &st = state->st;
+    if (pool < 2 || row_offset < 0 || skip_top < 0 || skip_bottom < 0 || skip_top + skip_bottom >= st.H ||
+        coarse_width < (st.W + pool - 1) / pool || coarse_height < (row_offset + st.H - skip_bottom + pool - 1) / pool)
+      rdb::fail("fill_blockmax: bad geometry");
+    st.blockmax_into(d_blockmax, coarse_width, coarse_height, pool, row_offset, skip_top, st.H - skip_bottom);
+    RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
+  });
 }
 
 int rdb200_dev_fill_prolong(rdb200_fill_state *state, const float *d_coarse, int32_t coarse_width, int32_t pool, int32_t row_offset,
                             int32_t *tiles_lowered) {
-  RDB_CAPI_TRY
-  if (!state) rdb::fail("fill_prolong: null state");
-  if (!d_coarse || pool < 2 || row_offset < 0) rdb::fail("fill_prolong: bad arguments");
-  rdb::Ctx &c = rdb::ctx();
-  rdb::DevBuf<int> cnt(1);
-  RDB_CK(cudaMemsetAsync(cnt.p, 0, sizeof(int), c.stream));
-  state->st.prolong_from(d_coarse, coarse_width, 0, 0, pool, row_offset, nullptr, 0, cnt.p);
-  int *h = (int *)c.pinned;
-  RDB_CK(cudaMemcpyAsync(h, cnt.p, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-  RDB_CK(cudaStreamSynchronize(c.stream));
-  if (tiles_lowered) *tiles_lowered = *h;
-  RDB_CAPI_END
+  return rdb::capi_call([&] {
+    if (!state) rdb::fail("fill_prolong: null state");
+    if (!d_coarse || pool < 2 || row_offset < 0) rdb::fail("fill_prolong: bad arguments");
+    rdb::Ctx &c = rdb::ctx();
+    rdb::DevBuf<int> cnt(1);
+    RDB_CK(cudaMemsetAsync(cnt.p, 0, sizeof(int), c.stream));
+    state->st.prolong_from(d_coarse, coarse_width, 0, 0, pool, row_offset, nullptr, 0, cnt.p);
+    int *h = (int *)c.pinned;
+    RDB_CK(cudaMemcpyAsync(h, cnt.p, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+    RDB_CK(cudaStreamSynchronize(c.stream));
+    if (tiles_lowered) *tiles_lowered = *h;
+  });
 }
 
 int rdb200_dev_fill_run(rdb200_fill_state *state, int32_t *changed_rows) {
-  RDB_CAPI_TRY
-  if (!state) rdb::fail("fill_run: null state");
-  state->st.activate_pending();
-  const int ch = state->st.run(rdb::ctx().params.fill_band_rounds);
-  if (changed_rows) *changed_rows = ch;
-  RDB_CAPI_END
+  return rdb::capi_call([&] {
+    if (!state) rdb::fail("fill_run: null state");
+    state->st.activate_pending();
+    const int ch = state->st.run(rdb::ctx().params.fill_band_rounds);
+    if (changed_rows) *changed_rows = ch;
+  });
 }
 
 int rdb200_dev_fill_read_row(rdb200_fill_state *state, int32_t y, float *d_row) {
-  RDB_CAPI_TRY
-  if (!state) rdb::fail("fill_read_row: null state");
-  state->st.read_row(y, d_row);
-  RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
-  RDB_CAPI_END
+  return rdb::capi_call([&] {
+    if (!state) rdb::fail("fill_read_row: null state");
+    state->st.read_row(y, d_row);
+    RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
+  });
 }
 
 int rdb200_dev_fill_update_row(rdb200_fill_state *state, int32_t y, const float *d_row) {
-  RDB_CAPI_TRY
-  if (!state) rdb::fail("fill_update_row: null state");
-  state->st.update_row(y, d_row);
-  RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
-  RDB_CAPI_END
+  return rdb::capi_call([&] {
+    if (!state) rdb::fail("fill_update_row: null state");
+    state->st.update_row(y, d_row);
+    RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
+  });
 }
 
 int rdb200_dev_fill_finish(rdb200_fill_state *state, float *d_out) {
-  RDB_CAPI_TRY
-  if (!state) rdb::fail("fill_finish: null state");
-  if (d_out) {
-    state->st.finish(d_out);
-    RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
-  }
-  delete state;
-  RDB_CAPI_END
+  return rdb::capi_call([&] {
+    if (!state) rdb::fail("fill_finish: null state");
+    if (d_out) {
+      state->st.finish(d_out);
+      RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
+    }
+    delete state;
+  });
 }
 
 }  // extern "C"

@@ -890,7 +890,6 @@ struct rdb200_flats_state {
 };
 
 namespace rdb {
-void capi_set_error(const char *msg);
 
 namespace {
 
@@ -1176,26 +1175,17 @@ void mgpu_d8_flow_directions_flats_band(const rdb200_comm *comm, float *d_dem, u
 
 }  // namespace rdb
 
-#define FLATS_TRY try {
-#define FLATS_END                      \
-  }                                    \
-  catch (const std::exception &e) {    \
-    rdb::capi_set_error(e.what());     \
-    return 1;                          \
-  }                                    \
-  return 0;
-
 extern "C" {
 
 int rdb200_dev_flats_begin(rdb200_flats_state **state, float *d_dem, int32_t width, int32_t height, float nodata,
                            int32_t ghost_top, int32_t ghost_bottom) {
-  FLATS_TRY
-  using namespace rdb;
-  ensure_init();
-  if (!state || !d_dem) fail("flats_begin: null pointer");
-  if (height - (ghost_top ? 1 : 0) - (ghost_bottom ? 1 : 0) < 1) fail("flats_begin: band has no owned rows");
-  *state = flats_begin(d_dem, width, height, nodata, ghost_top, ghost_bottom);
-  FLATS_END
+  return rdb::capi_call([&] {
+    using namespace rdb;
+    ensure_init();
+    if (!state || !d_dem) fail("flats_begin: null pointer");
+    if (height - (ghost_top ? 1 : 0) - (ghost_bottom ? 1 : 0) < 1) fail("flats_begin: band has no owned rows");
+    *state = flats_begin(d_dem, width, height, nodata, ghost_top, ghost_bottom);
+  });
 }
 
 // device addresses of the state arrays the caller moves across seams:
@@ -1204,61 +1194,51 @@ int rdb200_dev_flats_begin(rdb200_flats_state **state, float *d_dem, int32_t wid
 //   out[2] outlet flag per root (uint8, indexed by cell index of the root)
 //   out[3] away levels, out[4] towards levels (int32 H x W), out[5] flat height per root (int32)
 int rdb200_dev_flats_arrays(rdb200_flats_state *s, uint64_t *out6) {
-  FLATS_TRY
-  if (!s || !out6) rdb::fail("flats_arrays: null pointer");
-  out6[0] = (uint64_t)s->ft.p;
-  out6[1] = (uint64_t)s->labels.p;
-  out6[2] = (uint64_t)s->rootflag.p;
-  out6[3] = (uint64_t)s->away.p;
-  out6[4] = (uint64_t)s->tw.p;
-  out6[5] = (uint64_t)s->Hh.p;
-  FLATS_END
+  return rdb::capi_call([&] {
+    if (!s || !out6) rdb::fail("flats_arrays: null pointer");
+    out6[0] = (uint64_t)s->ft.p;
+    out6[1] = (uint64_t)s->labels.p;
+    out6[2] = (uint64_t)s->rootflag.p;
+    out6[3] = (uint64_t)s->away.p;
+    out6[4] = (uint64_t)s->tw.p;
+    out6[5] = (uint64_t)s->Hh.p;
+  });
 }
 
 int rdb200_dev_flats_edges(rdb200_flats_state *s) {
-  FLATS_TRY
-  rdb::flats_edges(s);
-  FLATS_END
+  return rdb::capi_call([&] { rdb::flats_edges(s); });
 }
 
 int rdb200_dev_flats_components(rdb200_flats_state *s) {
-  FLATS_TRY
-  rdb::flats_components(s);
-  FLATS_END
+  return rdb::capi_call([&] { rdb::flats_components(s); });
 }
 
 int rdb200_dev_flats_labels(rdb200_flats_state *s) {
-  FLATS_TRY
-  rdb::flats_labels(s);
-  FLATS_END
+  return rdb::capi_call([&] { rdb::flats_labels(s); });
 }
 
 int rdb200_dev_flats_gradient_begin(rdb200_flats_state *s, int32_t away, rdb200_fill_state **dist_state) {
-  FLATS_TRY
-  if (!dist_state) rdb::fail("flats_gradient_begin: null pointer");
-  *dist_state = rdb::flats_gradient_begin(s, away != 0);
-  FLATS_END
+  return rdb::capi_call([&] {
+    if (!dist_state) rdb::fail("flats_gradient_begin: null pointer");
+    *dist_state = rdb::flats_gradient_begin(s, away != 0);
+  });
 }
 
 int rdb200_dev_flats_gradient_end(rdb200_flats_state *s, int32_t away, rdb200_fill_state *dist_state) {
-  FLATS_TRY
-  rdb::flats_gradient_end(s, away != 0, dist_state);
-  FLATS_END
+  return rdb::capi_call([&] { rdb::flats_gradient_end(s, away != 0, dist_state); });
 }
 
 int rdb200_dev_flats_apply(rdb200_flats_state *s) {
-  FLATS_TRY
-  rdb::flats_apply(s);
-  FLATS_END
+  return rdb::capi_call([&] { rdb::flats_apply(s); });
 }
 
 int rdb200_dev_flats_finish(rdb200_flats_state *s) {
-  FLATS_TRY
-  if (s) {
-    RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
-    delete s;
-  }
-  FLATS_END
+  return rdb::capi_call([&] {
+    if (s) {
+      RDB_CK(cudaStreamSynchronize(rdb::ctx().stream));
+      delete s;
+    }
+  });
 }
 
 }  // extern "C"
