@@ -493,6 +493,58 @@ RDB200_API int rdb200_mgpu_flow_accumulation_props_f64(const rdb200_comm *comm, 
                                                        int32_t width, int32_t local_rows, int32_t ghost_top, int32_t ghost_bottom,
                                                        int32_t *exchange_rounds);
 
+/* float64 bands: the entry points above with double elevations and a double NoData, same band convention, argument
+ * checks (all before any communication) and result: the owned rows equal the single-GPU float64 entry point on the
+ * whole raster (rdb200_dev_*_f64), bit for bit where the float32 band call is bit for bit against its single-GPU twin.
+ * The fill, pit_mask, HasDepressions, ResolveFlatsEpsilon and FA_D8 / FA_D4 run the float32 band drivers on float keys
+ * kappa_G that every band shares: the cast to float when every band is float-exact, else global ranks built over the
+ * rank chain (DESIGN §0.1).  The ranks cap the distinct values of all bands together at 2^31 - 2^25; a raster above it
+ * fails on every rank before any stage runs.  The flow metrics, D-infinity / MFD accumulation and the terrain
+ * attributes run the double kernels on bands whose ghost rows were exchanged.
+ *   fill_depressions_*_f64     ghost rows ignored on entry, the neighbours' filled edge rows on return
+ *   pit_mask_*_f64, has_depressions_*_f64   d_band not modified, its ghost rows not read
+ *   resolve_flats_epsilon_f64  ghost rows not read on entry, the neighbours' resolved edge rows on return
+ *   fm_method_f64, terrain_attribute_f64   ghost rows of d_band_dem refreshed, as the float32 calls do
+ *   fa_method_f64_f64          methods as rdb200_mgpu_fa_method_f32_f64; ghost rows of d_band_dem not read */
+RDB200_API int rdb200_mgpu_fill_depressions_d8_f64(const rdb200_comm *comm, double *d_band, int32_t width, int32_t local_rows,
+                                                   int32_t ghost_top, int32_t ghost_bottom, int32_t row0, int32_t height,
+                                                   int32_t *exchange_rounds);
+RDB200_API int rdb200_mgpu_fill_depressions_d4_f64(const rdb200_comm *comm, double *d_band, int32_t width, int32_t local_rows,
+                                                   int32_t ghost_top, int32_t ghost_bottom, int32_t row0, int32_t height,
+                                                   int32_t *exchange_rounds);
+RDB200_API int rdb200_mgpu_pit_mask_d8_f64(const rdb200_comm *comm, const double *d_band, uint8_t *d_band_mask, int32_t width,
+                                           int32_t local_rows, double nodata, int32_t ghost_top, int32_t ghost_bottom, int32_t row0,
+                                           int32_t height);
+RDB200_API int rdb200_mgpu_pit_mask_d4_f64(const rdb200_comm *comm, const double *d_band, uint8_t *d_band_mask, int32_t width,
+                                           int32_t local_rows, double nodata, int32_t ghost_top, int32_t ghost_bottom, int32_t row0,
+                                           int32_t height);
+RDB200_API int rdb200_mgpu_has_depressions_d8_f64(const rdb200_comm *comm, const double *d_band, int32_t width, int32_t local_rows,
+                                                  int32_t ghost_top, int32_t ghost_bottom, int32_t row0, int32_t height,
+                                                  int32_t *out);
+RDB200_API int rdb200_mgpu_has_depressions_d4_f64(const rdb200_comm *comm, const double *d_band, int32_t width, int32_t local_rows,
+                                                  int32_t ghost_top, int32_t ghost_bottom, int32_t row0, int32_t height,
+                                                  int32_t *out);
+RDB200_API int rdb200_mgpu_resolve_flats_epsilon_f64(const rdb200_comm *comm, double *d_band, int32_t width, int32_t local_rows,
+                                                     double nodata, int32_t ghost_top, int32_t ghost_bottom,
+                                                     int32_t *seam_iterations);
+RDB200_API int rdb200_mgpu_fm_method_f64(const rdb200_comm *comm, int32_t method, double *d_band_dem, float *d_band_props9,
+                                         int32_t width, int32_t local_rows, double nodata, int32_t ghost_top, int32_t ghost_bottom,
+                                         double xparam);
+RDB200_API int rdb200_mgpu_terrain_attribute_f64(const rdb200_comm *comm, int32_t attribute, double *d_band_dem, float *d_band_out,
+                                                 int32_t width, int32_t local_rows, double nodata_in, float nodata_out, float zscale,
+                                                 double cell_x, double cell_y, int32_t ghost_top, int32_t ghost_bottom);
+RDB200_API int rdb200_mgpu_fa_method_f64_f64(const rdb200_comm *comm, const double *d_band_dem, double *d_band_accum_inout,
+                                             int32_t width, int32_t local_rows, double nodata, int32_t ghost_top,
+                                             int32_t ghost_bottom, int32_t method, double xparam, int32_t accum_is_ones,
+                                             int32_t *exchange_rounds);
+/* DIAGNOSTIC, not part of the stable interface (as rdb200_f64_order_keys): kappa_G of the owned rows into d_band_keys
+ * (local_rows x width; its ghost rows receive the neighbours' keys), *nodata_key = kappa_G(nodata) (the key of a cell
+ * equal to nodata in any band; else as rdb200_f64_order_keys), *ranked = 0 for the cast to float, 1 for global ranks
+ * (__uint_as_float(0x00800000 + r), r(v) = sum over the bands of their distinct values below v).  Collective. */
+RDB200_API int rdb200_mgpu_f64_order_keys(const rdb200_comm *comm, const double *d_band, float *d_band_keys, int32_t width,
+                                          int32_t local_rows, double nodata, int32_t ghost_top, int32_t ghost_bottom,
+                                          float *nodata_key, int32_t *ranked);
+
 /* ---- row-band (multi-GPU) fill: one band per GPU, halo rows exchanged by the caller -- */
 /* The band raster handed in is (band_rows + ghost rows) x width.  Its first and last rows are
  * boundary conditions that the solver never changes: a real raster border row, or a ghost

@@ -140,6 +140,17 @@ SIGNATURES = {
     "rdb200_mgpu_fm_method_f32": [_vp, _i32, _vp, _vp, _i32, _i32, _f32, _i32, _i32, C.c_double],
     "rdb200_mgpu_terrain_attribute_f32": [_vp, _i32, _vp, _vp, _i32, _i32, _f32, _f32, _f32, C.c_double, C.c_double, _i32, _i32],
     "rdb200_mgpu_flow_accumulation_props_f64": [_vp, _vp, _vp, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_mgpu_fill_depressions_d8_f64": [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_mgpu_fill_depressions_d4_f64": [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_mgpu_pit_mask_d8_f64": [_vp, _vp, _vp, _i32, _i32, _f64, _i32, _i32, _i32, _i32],
+    "rdb200_mgpu_pit_mask_d4_f64": [_vp, _vp, _vp, _i32, _i32, _f64, _i32, _i32, _i32, _i32],
+    "rdb200_mgpu_has_depressions_d8_f64": [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_mgpu_has_depressions_d4_f64": [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_mgpu_resolve_flats_epsilon_f64": [_vp, _vp, _i32, _i32, _f64, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_mgpu_fm_method_f64": [_vp, _i32, _vp, _vp, _i32, _i32, _f64, _i32, _i32, _f64],
+    "rdb200_mgpu_terrain_attribute_f64": [_vp, _i32, _vp, _vp, _i32, _i32, _f64, _f32, _f32, _f64, _f64, _i32, _i32],
+    "rdb200_mgpu_fa_method_f64_f64": [_vp, _vp, _vp, _i32, _i32, _f64, _i32, _i32, _i32, _f64, _i32, C.POINTER(_i32)],
+    "rdb200_mgpu_f64_order_keys": [_vp, _vp, _vp, _i32, _i32, _f64, _i32, _i32, C.POINTER(_f32), C.POINTER(_i32)],
     "rdb200_dev_fill_begin": [C.POINTER(_vp), _vp, _i32, _i32],
     "rdb200_dev_fill_begin_lifted": [C.POINTER(_vp), _vp, _i32, _i32, _vp, _i32, _i32, _i32],
     "rdb200_dev_maxpool_rows_f32": [_vp, _i32, _i32, _i32, _i32, _vp, _i32, _i32],

@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "librichdem_b200.so")
 SOURCES = ["capi.cu", "comm.cu", "fill.cu", "flats.cu", "flowdirs.cu", "accum.cu", "terrain.cu", "attributes.cu", "depressions.cu",
-           "f64.cu"]
+           "f64.cu", "f64_band.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
     *GENCODE,

@@ -471,6 +471,35 @@ static int mgpu_has_depressions(const rdb200_comm *comm, const float *d_band, in
   return rc;
 }
 
+// float64 bands: every argument is checked before kappa_G's first collective
+static int mgpu_fill_f64(const rdb200_comm *comm, double *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb, int32_t row0,
+                         int32_t height, int32_t *exchange_rounds, bool topo4) {
+  int xr = 0;
+  const int rc = raster_call(Side::device, "mgpu_fill: null pointer", {d_band}, w, rows, [&](Arrays &, size_t) {
+    mgpu_fill_f64_band(comm, d_band, w, rows, gt, gb, row0, height, &xr, topo4);
+  });
+  if (rc == 0 && exchange_rounds) *exchange_rounds = xr;
+  return rc;
+}
+
+static int mgpu_pit_mask_f64(const rdb200_comm *comm, const double *d_band, uint8_t *d_band_mask, int32_t w, int32_t rows,
+                             double nodata, int32_t gt, int32_t gb, int32_t row0, int32_t height, bool topo4) {
+  return raster_call(Side::device, "mgpu_pit_mask: null pointer", {comm, d_band, d_band_mask}, w, rows, [&](Arrays &, size_t) {
+    mgpu_pit_mask_f64_band(comm, d_band, d_band_mask, w, rows, nodata, gt, gb, row0, height, topo4);
+  });
+}
+
+static int mgpu_has_depressions_f64(const rdb200_comm *comm, const double *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb,
+                                    int32_t row0, int32_t height, int32_t *out, bool topo4) {
+  bool any = false;
+  const int rc = raster_call(Side::device, "mgpu_has_depressions: null pointer", {comm, d_band, out}, w, rows,
+                             [&](Arrays &, size_t) {
+                               any = mgpu_has_depressions_f64_band(comm, d_band, w, rows, gt, gb, row0, height, topo4);
+                             });
+  if (rc == 0) *out = any ? 1 : 0;
+  return rc;
+}
+
 }  // namespace rdb
 
 using namespace rdb;
@@ -564,6 +593,7 @@ int rdb200_set_param(const char *name, int64_t value) {
     else if (n == "accum_walk_ahead") p.accum_walk_ahead = value;
     else if (n == "accum_dinf_stats") p.accum_dinf_stats = value;
     else if (n == "accum_dinf_wait") p.accum_dinf_wait = value;
+    else if (n == "f64_band_rank_cap") p.f64_band_rank_cap = value;
     else fail("rdb200_set_param: unknown parameter '%s'", name);
   });
 }
@@ -944,6 +974,102 @@ int rdb200_mgpu_d8_flow_accum_u8_i32(const rdb200_comm *comm, const uint8_t *d_b
   const int rc = raster_call(Side::device, "mgpu_d8_flow_accum: null pointer", {comm, d_band_dirs, d_band_area}, w, rows,
                              [&](Arrays &, size_t) { mgpu_d8_flow_accum_band(comm, d_band_dirs, d_band_area, w, rows, gt, gb, &xr); });
   if (rc == 0 && exchange_rounds) *exchange_rounds = xr;
+  return rc;
+}
+
+// ---- float64 row bands (f64_band.cu): the float32 band drivers on kappa_G, and the double flow metrics and attributes --
+
+int rdb200_mgpu_fill_depressions_d8_f64(const rdb200_comm *comm, double *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb,
+                                        int32_t row0, int32_t height, int32_t *exchange_rounds) {
+  return mgpu_fill_f64(comm, d_band, w, rows, gt, gb, row0, height, exchange_rounds, false);
+}
+int rdb200_mgpu_fill_depressions_d4_f64(const rdb200_comm *comm, double *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb,
+                                        int32_t row0, int32_t height, int32_t *exchange_rounds) {
+  return mgpu_fill_f64(comm, d_band, w, rows, gt, gb, row0, height, exchange_rounds, true);
+}
+int rdb200_mgpu_pit_mask_d8_f64(const rdb200_comm *comm, const double *d_band, uint8_t *d_band_mask, int32_t w, int32_t rows,
+                                double nodata, int32_t gt, int32_t gb, int32_t row0, int32_t height) {
+  return mgpu_pit_mask_f64(comm, d_band, d_band_mask, w, rows, nodata, gt, gb, row0, height, false);
+}
+int rdb200_mgpu_pit_mask_d4_f64(const rdb200_comm *comm, const double *d_band, uint8_t *d_band_mask, int32_t w, int32_t rows,
+                                double nodata, int32_t gt, int32_t gb, int32_t row0, int32_t height) {
+  return mgpu_pit_mask_f64(comm, d_band, d_band_mask, w, rows, nodata, gt, gb, row0, height, true);
+}
+int rdb200_mgpu_has_depressions_d8_f64(const rdb200_comm *comm, const double *d_band, int32_t w, int32_t rows, int32_t gt,
+                                       int32_t gb, int32_t row0, int32_t height, int32_t *out) {
+  return mgpu_has_depressions_f64(comm, d_band, w, rows, gt, gb, row0, height, out, false);
+}
+int rdb200_mgpu_has_depressions_d4_f64(const rdb200_comm *comm, const double *d_band, int32_t w, int32_t rows, int32_t gt,
+                                       int32_t gb, int32_t row0, int32_t height, int32_t *out) {
+  return mgpu_has_depressions_f64(comm, d_band, w, rows, gt, gb, row0, height, out, true);
+}
+
+int rdb200_mgpu_resolve_flats_epsilon_f64(const rdb200_comm *comm, double *d_band, int32_t w, int32_t rows, double nodata,
+                                          int32_t gt, int32_t gb, int32_t *seam_iterations) {
+  int it = 0;
+  const int rc = raster_call(Side::device, "mgpu_resolve_flats: null pointer", {comm, d_band}, w, rows,
+                             [&](Arrays &, size_t) { mgpu_resolve_flats_f64_band(comm, d_band, w, rows, nodata, gt, gb, &it); });
+  if (rc == 0 && seam_iterations) *seam_iterations = it;
+  return rc;
+}
+
+int rdb200_mgpu_fm_method_f64(const rdb200_comm *comm, int32_t method, double *d_band_dem, float *d_band_props9, int32_t w,
+                              int32_t rows, double nodata, int32_t gt, int32_t gb, double xparam) {
+  return raster_call(
+      Side::device, "mgpu_fm_method: null pointer", {d_band_props9, comm, d_band_dem}, w, rows,
+      [&] {
+        check_band_args("mgpu_fm_method", comm, d_band_dem, w, rows, gt, gb);
+        if (method < 0 || method > 4) fail("unknown flow metric %d", method);
+      },
+      [&](Arrays &, size_t) {
+        exchange_band_rows(comm, d_band_dem, sizeof(double), w, rows, gt, gb);
+        fm_method_f64_dev(method, d_band_dem, d_band_props9, w, rows, nodata, xparam);
+      });
+}
+
+int rdb200_mgpu_terrain_attribute_f64(const rdb200_comm *comm, int32_t attribute, double *d_band_dem, float *d_band_out, int32_t w,
+                                      int32_t rows, double nodata_in, float nodata_out, float zscale, double cell_x, double cell_y,
+                                      int32_t gt, int32_t gb) {
+  return raster_call(
+      Side::device, "mgpu_terrain_attribute: null pointer", {d_band_out, comm, d_band_dem}, w, rows,
+      [&] {
+        check_band_args("mgpu_terrain_attribute", comm, d_band_dem, w, rows, gt, gb);
+        if (attribute < RDB200_TA_SLOPE_RISERUN || attribute > RDB200_TA_PROFILE_CURVATURE)
+          fail("unknown terrain attribute %d", attribute);
+        if (!(cell_x > 0) || !(cell_y > 0))
+          fail("terrain attribute: cell lengths must be positive (got %g x %g)", cell_x, cell_y);
+      },
+      [&](Arrays &, size_t) {
+        exchange_band_rows(comm, d_band_dem, sizeof(double), w, rows, gt, gb);
+        terrain_attribute_f64_dev(attribute, d_band_dem, d_band_out, w, rows, nodata_in, nodata_out, zscale, cell_x, cell_y);
+      });
+}
+
+int rdb200_mgpu_fa_method_f64_f64(const rdb200_comm *comm, const double *d_dem, double *d_accum, int32_t w, int32_t rows,
+                                  double nodata, int32_t gt, int32_t gb, int32_t method, double xparam, int32_t ones,
+                                  int32_t *exchange_rounds) {
+  int xr = 0;
+  const int rc = raster_call(
+      Side::device, "mgpu_fa: null pointer", {comm, d_dem, d_accum}, w, rows,
+      [&] {
+        check_band_args("mgpu_fa", comm, d_dem, w, rows, gt, gb);
+        check_fa_method(method, xparam);
+      },
+      [&](Arrays &, size_t) { mgpu_fa_f64_band(comm, d_dem, d_accum, w, rows, nodata, gt, gb, method, xparam, ones != 0, &xr); });
+  if (rc == 0 && exchange_rounds) *exchange_rounds = xr;
+  return rc;
+}
+
+int rdb200_mgpu_f64_order_keys(const rdb200_comm *comm, const double *d_band, float *d_band_keys, int32_t w, int32_t rows,
+                               double nodata, int32_t gt, int32_t gb, float *nodata_key, int32_t *ranked) {
+  float nd = 0;
+  int r = 0;
+  const int rc = raster_call(
+      Side::device, "mgpu_f64_order_keys: null pointer", {comm, d_band, d_band_keys}, w, rows,
+      [&] { check_band_args("mgpu_f64_order_keys", comm, d_band, w, rows, gt, gb); },
+      [&](Arrays &, size_t) { nd = mgpu_f64_keys_dev(comm, d_band, d_band_keys, w, rows, gt, gb, nodata, nullptr, &r); });
+  if (rc == 0 && nodata_key) *nodata_key = nd;
+  if (rc == 0 && ranked) *ranked = r;
   return rc;
 }
 

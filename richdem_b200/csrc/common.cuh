@@ -102,6 +102,7 @@ struct Params {
   int64_t accum_walk_lanes = 1;   // unit-weight D8 walk (row bands): persistent always-busy lanes fed from per-warp source queues
   int64_t accum_threads = 256;
   int64_t accum_budget = 0;  // cells one thread follows per level in the multi-receiver accumulation (0: 4)
+  int64_t f64_band_rank_cap = 0;  // float64 row bands: distinct values the bands may hold in all (0: 2^31 - 2^25)
 };
 
 struct WsBlock {
@@ -186,12 +187,14 @@ void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, in
 // method: 0 D8, 1 Tarboton, 2 D4, 3 Holmgren (xparam; Quinn = 1.0), 4 Freeman (xparam)
 void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, int w, int hloc, float nodata, int gt, int gb,
                   int method, double xparam, bool ones, int *xrounds);
+void check_fa_method(int method, double xparam);  // an unknown method, or a non-finite exponent, is an error
 // FlowAccumulation(props, accum) of caller-supplied 9-float proportions; the ghost rows of d_props are overwritten with the
 // neighbours' edge rows
 void mgpu_flow_accumulation_props_band(const rdb200_comm *comm, float *d_props, double *d_accum, int w, int hloc, int gt, int gb,
                                        int *xrounds);
+// d_mask_out (w x hloc, may be null): write the increment mask there and leave the elevations and their ghost rows alone
 void mgpu_resolve_flats_band(const rdb200_comm *comm, float *d_local, int w, int hloc, float nodata, int gt, int gb,
-                             int *seam_iters);
+                             int *seam_iters, int32_t *d_mask_out = nullptr);
 void mgpu_d8_flow_directions_flats_band(const rdb200_comm *comm, float *d_dem, uint8_t *d_dirs, int w, int hloc, float nodata,
                                         int gt, int gb, bool alter, int *seam_iters);
 void mgpu_d8_flow_accum_band(const rdb200_comm *comm, const uint8_t *d_dirs, int32_t *d_area, int w, int hloc, int gt, int gb,
@@ -249,5 +252,36 @@ void fm_method_f64_dev(int method, const double *d_dem, float *d_props, int w, i
 void fa_tarboton_f64_dev(const double *d_dem, double *d_accum, int w, int h, double nodata, bool ones);
 void terrain_attribute_f64_dev(int attribute_id, const double *d_dem, float *d_out, int w, int h, double nodata_in,
                                float nodata_out, float zscale, double cell_x, double cell_y);
+void f64_apply_ulps_dev(double *d_z, const int32_t *d_mask, int w, int h);
+int32_t read_i32(const int32_t *d_value);  // one device int, read back after the library's stream
+
+// ---- float64 row bands: kappa_G, one key map shared by every band (f64.cu), and the band drivers (f64_band.cu) ----
+// What a band keeps of kappa_G for kappa_G^-1: D_b (vals: [count | values], cap + 1 slots, cap = max over the bands of
+// |D_b|) and r(D_b) (keys, strictly increasing), m = |D_b|.  ranked = 0: the cast route, nothing kept.
+struct BandKeys {
+  bool ranked = false;
+  size_t m = 0, cap = 0;
+  DevBuf<double> vals;
+  DevBuf<uint32_t> keys;
+};
+// kappa_G of the owned rows of a double band into d_band_keys (same layout); its ghost rows receive the neighbours' owned
+// keys.  Collective.  Returns kappa_G(nodata); inv (may be null) receives what kappa_G^-1 needs, *ranked the route.
+float mgpu_f64_keys_dev(const rdb200_comm *comm, const double *d_band, float *d_band_keys, int w, int hloc, int gt, int gb,
+                        double nodata, BandKeys *inv, int *ranked);
+// the fill's write-back over bands: owned cells whose key k0 -> kf was raised take kappa_G^-1(kf).  Collective.
+void mgpu_f64_writeback_dev(const rdb200_comm *comm, const BandKeys &inv, double *d_band, const float *k0, const float *kf, int w,
+                            int hloc, int gt, int gb);
+void check_mask_band(const char *what, const rdb200_comm *comm, const void *d_band, int w, int hloc, int gt, int gb, int row0,
+                     int H);
+void mgpu_fill_f64_band(const rdb200_comm *comm, double *d_band, int w, int hloc, int gt, int gb, int row0, int H, int *xrounds,
+                        bool topo4);
+void mgpu_pit_mask_f64_band(const rdb200_comm *comm, const double *d_band, uint8_t *d_mask, int w, int hloc, double nodata, int gt,
+                            int gb, int row0, int H, bool topo4);
+bool mgpu_has_depressions_f64_band(const rdb200_comm *comm, const double *d_band, int w, int hloc, int gt, int gb, int row0, int H,
+                                   bool topo4);
+void mgpu_resolve_flats_f64_band(const rdb200_comm *comm, double *d_band, int w, int hloc, double nodata, int gt, int gb,
+                                 int *seam_iters);
+void mgpu_fa_f64_band(const rdb200_comm *comm, const double *d_dem, double *d_accum, int w, int hloc, double nodata, int gt, int gb,
+                      int method, double xparam, bool ones, int *xrounds);
 
 }  // namespace rdb

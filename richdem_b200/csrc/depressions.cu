@@ -172,8 +172,8 @@ bool has_depressions_dev(const float *d_dem, int w, int h, bool topo4) {
 // The band fill runs on a copy of the local raster (mgpu_fill_band ignores the ghost rows on entry), so d_band is not
 // modified; the compare then runs on the owned rows.  A raster without interior cells is its own fill (no band fill:
 // every rank sees the same width and height, so all skip it together).
-static void check_mask_band(const char *what, const rdb200_comm *comm, const float *d_band, int w, int hloc, int gt, int gb,
-                            int row0, int H) {
+void check_mask_band(const char *what, const rdb200_comm *comm, const void *d_band, int w, int hloc, int gt, int gb, int row0,
+                     int H) {
   check_band_args(what, comm, d_band, w, hloc, gt, gb);
   if (row0 < 0 || row0 + hloc > H) fail("%s: rows [%d, %d) are outside the raster (%d rows)", what, row0, row0 + hloc, H);
   if (w >= 3 && H >= 3 && hloc < 3) fail("%s: band too small (%d x %d); the band fill needs three local rows", what, w, hloc);

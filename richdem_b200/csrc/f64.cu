@@ -8,6 +8,7 @@
 // compare equal, the float engine on kappa(Z) takes the control flow the double template takes on Z, and every value it
 // copies is kappa of the value the double run copies.  This file builds kappa(Z) (the only new hot path), maps a filled
 // key raster back to doubles, and applies the flats' increment mask as double ulps.  The float engines run unchanged.
+// Over row bands the same engines run on kappa_G, one map shared by every band (the second half of this file).
 //
 // kappa, chosen by looking at the input:
 //   case 1  every value is NaN, +-inf or a float-exact double with |z| < FLT_MAX (a widened float raster):
@@ -280,7 +281,8 @@ __global__ void __launch_bounds__(256) scan_apply_kernel(uint32_t *a, size_t m, 
 __global__ void __launch_bounds__(256) rank_scatter_kernel(const uint64_t *__restrict__ ks, const uint32_t *__restrict__ is,
                                                            const double *__restrict__ z, size_t n,
                                                            const uint32_t *__restrict__ sums, float *__restrict__ key,
-                                                           double *__restrict__ table, double nodata, uint32_t *nd_key) {
+                                                           double *__restrict__ table, double nodata, uint32_t *nd_key,
+                                                           uint32_t *distinct) {
   __shared__ uint32_t ws[8];
   const HeadSrc head{ks, z};
   const size_t base = (size_t)blockIdx.x * SORT_TILE;
@@ -302,6 +304,7 @@ __global__ void __launch_bounds__(256) rank_scatter_kernel(const uint64_t *__res
       const float f = rank_key(v, rank);
       key[idx] = f;
       if (h && table) table[rank] = v;
+      if (distinct && i == n - 1) *distinct = rank + 1u;
       if (v == nodata) {
         found = 1;
         nd_bits = __float_as_uint(f);
@@ -379,25 +382,13 @@ float nodata_image(double nodata) {
   return host_bits_float(0x7fc00000u);
 }
 
-}  // namespace
-
-float f64_keys_dev(const double *d_z, float *d_key, size_t n, double nodata, DevBuf<double> *table, int *ranked) {
+// case 2 of kappa: d_key = the dense-rank keys, *d_nd = the key of a cell equal to nodata (left alone without one),
+// *table (may be null) = the sorted distinct values, *d_distinct (may be null) = their number.  hist: 2048 device words.
+void rank_route(const double *d_z, float *d_key, size_t n, double nodata, DevBuf<double> *table, uint32_t *d_nd,
+                uint32_t *d_distinct, uint32_t *d_hist) {
   Ctx &c = ctx();
-  DevBuf<uint32_t> flags(2 + 8 * 256);  // [0] inexact, [1] nodata key, [2..] digit histograms
-  uint32_t *d_inexact = flags.p, *d_nd = flags.p + 1, *d_hist = flags.p + 2;
-  RDB_CK(cudaMemsetAsync(d_inexact, 0, sizeof(uint32_t), c.stream));
-  RDB_CK(cudaMemsetAsync(d_nd, 0xff, sizeof(uint32_t), c.stream));
-  f64_cast_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, d_key, n, nodata, (int *)d_inexact, d_nd);
-  RDB_CK(cudaGetLastError());
-  count_launch();
-  uint32_t *hb = (uint32_t *)c.pinned;  // 2 + 2048 words fit the 64 KiB pinned scratch
-  RDB_CK(cudaMemcpyAsync(hb, flags.p, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
-  RDB_CK(cudaStreamSynchronize(c.stream));
-  if (ranked) *ranked = hb[0] != 0;
-  if (hb[0] == 0) return hb[1] != NO_KEY ? host_bits_float(hb[1]) : nodata_image(nodata);
-
-  // case 2: which digits differ between keys
-  RDB_CK(cudaMemsetAsync(d_nd, 0xff, sizeof(uint32_t), c.stream));
+  uint32_t *hb = (uint32_t *)c.pinned;  // 2048 words fit the 64 KiB pinned scratch
+  // which digits differ between keys
   RDB_CK(cudaMemsetAsync(d_hist, 0, 8 * 256 * sizeof(uint32_t), c.stream));
   digit_hist_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, n, d_hist);
   RDB_CK(cudaGetLastError());
@@ -437,9 +428,29 @@ float f64_keys_dev(const double *d_z, float *d_key, size_t n, double nodata, Dev
   if (table) table->alloc(n);
   chunk_sums_dev(HeadSrc{ks, zsrc}, n, sums.p, tiles);
   rank_scatter_kernel<<<(unsigned)tiles, 256, 0, c.stream>>>(ks, is, zsrc, n, sums.p, d_key, table ? table->p : nullptr, nodata,
-                                                             d_nd);
+                                                             d_nd, d_distinct);
   RDB_CK(cudaGetLastError());
   count_launch();
+}
+
+}  // namespace
+
+float f64_keys_dev(const double *d_z, float *d_key, size_t n, double nodata, DevBuf<double> *table, int *ranked) {
+  Ctx &c = ctx();
+  DevBuf<uint32_t> flags(2 + 8 * 256);  // [0] inexact, [1] nodata key, [2..] digit histograms
+  uint32_t *d_inexact = flags.p, *d_nd = flags.p + 1, *d_hist = flags.p + 2;
+  RDB_CK(cudaMemsetAsync(d_inexact, 0, sizeof(uint32_t), c.stream));
+  RDB_CK(cudaMemsetAsync(d_nd, 0xff, sizeof(uint32_t), c.stream));
+  f64_cast_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, d_key, n, nodata, (int *)d_inexact, d_nd);
+  RDB_CK(cudaGetLastError());
+  count_launch();
+  uint32_t *hb = (uint32_t *)c.pinned;
+  RDB_CK(cudaMemcpyAsync(hb, flags.p, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  if (ranked) *ranked = hb[0] != 0;
+  if (hb[0] == 0) return hb[1] != NO_KEY ? host_bits_float(hb[1]) : nodata_image(nodata);
+  RDB_CK(cudaMemsetAsync(d_nd, 0xff, sizeof(uint32_t), c.stream));
+  rank_route(d_z, d_key, n, nodata, table, d_nd, nullptr, d_hist);
   RDB_CK(cudaMemcpyAsync(hb, d_nd, sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
   RDB_CK(cudaStreamSynchronize(c.stream));
   return hb[0] != NO_KEY ? host_bits_float(hb[0]) : nodata_image(nodata);
@@ -514,6 +525,387 @@ void fa_d8_f64_dev(const double *d_z, double *d_accum, int w, int h, double noda
   DevBuf<float> key(n);
   const float nd = f64_keys_dev(d_z, key.p, n, nodata, nullptr, nullptr);
   fa_fused_dev(key.p, d_accum, w, h, nd, ones, false);
+}
+
+// ---- kappa_G: one key map for a raster cut into row bands (DESIGN §0.1 "kappa over row bands") ---------------------
+// Cast route when every band is float-exact.  Otherwise band b sorts its owned values into D_b (its sorted distinct
+// values other than NaN, +-inf and +-DBL_MAX) and every value v gets the key r(v) = sum over the bands c of
+// |{u in D_c : u < v}|: strictly increasing on the raster's values (v < v' and v in D_a give |{u in D_a : u < v'}| >
+// |{u in D_a : u < v}|), equal for equal values, and the same in every band that holds v.  The own band's term is the
+// local dense rank; the other bands' terms come from passing every D_c along the rank chain, G - 1 steps in each
+// direction, and counting with a merge-path kernel how many received values lie below each element of D_b.
+
+namespace {
+
+constexpr int MERGE_ITEMS = 8;
+constexpr int MERGE_TILE = 256 * MERGE_ITEMS;  // merged entries per block of the count kernel
+
+__device__ __forceinline__ bool rank_form(float k) { return k == k && fabsf(k) < FLT_MAX; }  // not a sentinel image
+
+// a message of the chain: [0] the entry count (int64 bits), then the values (and, for kappa_G^-1, the keys after them)
+__device__ __forceinline__ size_t msg_count(const double *msg) { return (size_t)__double_as_longlong(msg[0]); }
+
+// merge path of sorted a (na) and b (nb), a first on ties: how many of the first d merged entries come from a
+__device__ __forceinline__ size_t merge_split(const double *a, size_t na, const double *b, size_t nb, size_t d) {
+  size_t lo = d > nb ? d - nb : 0, hi = d < na ? d : na;
+  while (lo < hi) {
+    const size_t mid = (lo + hi) / 2;
+    if (a[mid] <= b[d - mid - 1]) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// cnt[i] += |{u in msg : u < a[i]}| for the sorted a (m values, no NaN) and the sorted values of a chain message.  Block
+// k takes merged entries [k T, (k+1) T): it finds its ranges of a and of the message by two merge-path searches, stages
+// them in shared memory (coalesced), and every thread merges 8 consecutive entries.  When an element of a is emitted,
+// the message entries merged before it are exactly those below it.
+__global__ void __launch_bounds__(256) merge_count_kernel(const double *__restrict__ a, size_t m, const double *__restrict__ msg,
+                                                          uint32_t *__restrict__ cnt) {
+  __shared__ double s[MERGE_TILE];
+  __shared__ size_t s_split[2];
+  const size_t mb = msg_count(msg);
+  const double *b = msg + 1;
+  const size_t total = m + mb, d0 = (size_t)blockIdx.x * MERGE_TILE;
+  if (d0 >= total) return;  // the whole block
+  const size_t d1 = d0 + MERGE_TILE < total ? d0 + MERGE_TILE : total;
+  if (threadIdx.x < 2) s_split[threadIdx.x] = merge_split(a, m, b, mb, threadIdx.x ? d1 : d0);
+  __syncthreads();
+  const size_t i0 = s_split[0], j0 = d0 - i0, i1 = s_split[1], j1 = d1 - i1;
+  const int na = (int)(i1 - i0), nb = (int)(j1 - j0);
+  for (int k = threadIdx.x; k < na + nb; k += blockDim.x) s[k] = k < na ? a[i0 + k] : b[j0 + (k - na)];
+  __syncthreads();
+  const int dt = (int)threadIdx.x * MERGE_ITEMS < na + nb ? (int)threadIdx.x * MERGE_ITEMS : na + nb;
+  int lo = dt > nb ? dt - nb : 0, hi = dt < na ? dt : na;
+  while (lo < hi) {
+    const int mid = (lo + hi) / 2;
+    if (s[mid] <= s[na + dt - mid - 1]) lo = mid + 1;
+    else hi = mid;
+  }
+  int i = lo, j = dt - lo;
+  for (int k = 0; k < MERGE_ITEMS && i + j < na + nb; k++) {
+    if (j >= nb || (i < na && s[i] <= s[na + j])) {
+      cnt[i0 + i] += (uint32_t)(j0 + j);
+      i++;
+    } else {
+      j++;
+    }
+  }
+}
+
+// the band's table: [0] first entry of D_b in the sorted distinct values (past -DBL_MAX and below), [1] |D_b|,
+// [2] |{u in D_b : u < nodata}|.  One thread.
+__global__ void band_table_bounds_kernel(const double *__restrict__ table, const uint32_t *__restrict__ distinct, double nodata,
+                                         long long *info) {
+  const size_t m = *distinct;
+  size_t lo = 0, hi = m;
+  const uint64_t klo = order_key(-DBL_MAX) + 1, khi = order_key(DBL_MAX);
+  while (lo < hi) {  // first entry above -DBL_MAX
+    const size_t mid = (lo + hi) / 2;
+    if (order_key(table[mid]) < klo) lo = mid + 1;
+    else hi = mid;
+  }
+  const size_t first = lo;
+  hi = m;
+  while (lo < hi) {  // first entry at DBL_MAX or above
+    const size_t mid = (lo + hi) / 2;
+    if (order_key(table[mid]) < khi) lo = mid + 1;
+    else hi = mid;
+  }
+  const size_t end = lo;
+  lo = first, hi = end;
+  while (lo < hi) {  // a NaN nodata counts nothing
+    const size_t mid = (lo + hi) / 2;
+    if (table[mid] < nodata) lo = mid + 1;
+    else hi = mid;
+  }
+  info[0] = (long long)first;
+  info[1] = (long long)(end - first);
+  info[2] = (long long)(lo - first);
+}
+
+__global__ void __launch_bounds__(256) iota_kernel(uint32_t *__restrict__ a, size_t n) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) a[i] = (uint32_t)i;
+}
+
+// local dense-rank keys -> global keys (lo: the table index of D_b[0]); sentinel images stay
+__global__ void __launch_bounds__(256) band_gather_kernel(float *__restrict__ key, size_t n, const uint32_t *__restrict__ r,
+                                                          uint32_t lo) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const float k = key[i];
+    if (rank_form(k)) key[i] = __uint_as_float(RANK_BASE + r[__float_as_uint(k) - RANK_BASE - lo]);
+  }
+}
+
+// index of key rr in the strictly increasing keys[0, m), or m
+__device__ __forceinline__ size_t find_key(const uint32_t *__restrict__ keys, size_t m, uint32_t rr) {
+  size_t lo = 0, hi = m;
+  while (lo < hi) {
+    const size_t mid = (lo + hi) / 2;
+    if (keys[mid] < rr) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo < m && keys[lo] == rr ? lo : m;
+}
+
+// kappa_G^-1 from the band's own table (r(D_b), D_b): cells the fill did not raise keep their bits; a raised cell whose
+// level is not in D_b is left pending for the chain pass
+__global__ void __launch_bounds__(256) band_writeback_kernel(double *__restrict__ z, const float *__restrict__ key0,
+                                                             const float *__restrict__ keyf, size_t n, const uint32_t *__restrict__ r,
+                                                             const double *__restrict__ vals, size_t m, uint8_t *__restrict__ pending,
+                                                             int *miss) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  int missed = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const float b = keyf[i];
+    uint8_t p = 0;
+    if (__float_as_uint(b) != __float_as_uint(key0[i])) {
+      if (!rank_form(b)) {
+        z[i] = key_value(b, vals);
+      } else {
+        const size_t at = find_key(r, m, __float_as_uint(b) - RANK_BASE);
+        if (at < m) z[i] = vals[at];
+        else p = 1, missed = 1;
+      }
+    }
+    pending[i] = p;
+  }
+  if (__syncthreads_or(missed) && threadIdx.x == 0) *miss = 1;
+}
+
+// the pending cells whose level a received table (values, then keys after cap values) holds
+__global__ void __launch_bounds__(256) band_lookup_kernel(double *__restrict__ z, const float *__restrict__ keyf, size_t n,
+                                                          uint8_t *__restrict__ pending, const double *__restrict__ msg, size_t cap,
+                                                          int *left) {
+  const size_t mb = msg_count(msg);
+  const double *vals = msg + 1;
+  const uint32_t *keys = reinterpret_cast<const uint32_t *>(msg + 1 + cap);
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  int still = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (!pending[i]) continue;
+    const size_t at = find_key(keys, mb, __float_as_uint(keyf[i]) - RANK_BASE);
+    if (at < mb) {
+      z[i] = vals[at];
+      pending[i] = 0;
+    } else {
+      still = 1;
+    }
+  }
+  if (left && __syncthreads_or(still) && threadIdx.x == 0) *left = 1;
+}
+
+// a kappa(nodata) that is a sentinel image, else 0
+float sentinel_image(double v) {
+  if (v != v) return host_bits_float(0x7fc00000u);
+  if (v == (double)INFINITY || v == -(double)INFINITY || v == DBL_MAX || v == -DBL_MAX) return nodata_image(v);
+  return 0.f;
+}
+
+// a chain message's header on the device
+void set_msg_count(double *d_msg, size_t count) {
+  Ctx &c = ctx();
+  int64_t *h = (int64_t *)c.pinned;
+  *h = (int64_t)count;
+  RDB_CK(cudaMemcpyAsync(d_msg, h, sizeof(int64_t), cudaMemcpyHostToDevice, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+}
+
+// Pass every band's message (slots doubles after the header) along the chain: G - 1 steps, each sending up what came
+// from below and down what came from above (the own message first); visit(msg) runs on each message received.  A side
+// without a neighbour receives nothing, so what it forwards has count 0.
+template <class Visit>
+void chain_pass(const rdb200_comm *comm, const double *d_own, size_t slots, Visit &&visit) {
+  Ctx &c = ctx();
+  const int rank = comm_rank(comm), world = comm_world(comm);
+  if (world == 1) return;
+  const size_t words = slots + 1;
+  DevBuf<double> bufs(4 * words);  // receive from above / below, two of each (the one received last is sent next)
+  RDB_CK(cudaMemsetAsync(bufs.p, 0, 4 * words * sizeof(double), c.stream));
+  double *from_up[2] = {bufs.p, bufs.p + words}, *from_dn[2] = {bufs.p + 2 * words, bufs.p + 3 * words};
+  const double *send_up = d_own, *send_dn = d_own;
+  for (int s = 0; s < world - 1; s++) {
+    double *ru = from_up[s & 1], *rd = from_dn[s & 1];
+    comm_exchange(comm, send_up, ru, send_dn, rd, words * sizeof(double));
+    if (rank > 0) visit(ru);
+    if (rank < world - 1) visit(rd);
+    send_dn = ru;  // what came from above goes on down, what came from below goes on up
+    send_up = rd;
+  }
+}
+
+}  // namespace
+
+int32_t read_i32(const int32_t *d) {
+  Ctx &c = ctx();
+  int32_t *h = (int32_t *)c.pinned;
+  RDB_CK(cudaMemcpyAsync(h, d, sizeof(int32_t), cudaMemcpyDeviceToHost, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  return *h;
+}
+
+float mgpu_f64_keys_dev(const rdb200_comm *comm, const double *d_band, float *d_band_keys, int w, int hloc, int gt, int gb,
+                        double nodata, BandKeys *inv, int *ranked) {
+  Ctx &c = ctx();
+  const int rank = comm_rank(comm), world = comm_world(comm);
+  gt = gt ? 1 : 0;
+  gb = gb ? 1 : 0;
+  const size_t n = (size_t)w * (hloc - gt - gb), off = (size_t)w * gt;
+  const double *d_z = d_band + off;
+  float *d_key = d_band_keys + off;
+  DevBuf<uint32_t> flags(4 + 8 * 256);  // [0] inexact, [1] nodata key, [2] distinct values, [3] spare, [4..] histograms
+  uint32_t *d_inexact = flags.p, *d_nd = flags.p + 1, *d_distinct = flags.p + 2, *d_hist = flags.p + 4;
+  RDB_CK(cudaMemsetAsync(d_inexact, 0, sizeof(uint32_t), c.stream));
+  RDB_CK(cudaMemsetAsync(d_nd, 0xff, sizeof(uint32_t), c.stream));
+  f64_cast_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, d_key, n, nodata, (int *)d_inexact, d_nd);
+  RDB_CK(cudaGetLastError());
+  count_launch();
+  uint32_t *hb = (uint32_t *)c.pinned;
+  RDB_CK(cudaMemcpyAsync(hb, flags.p, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  const uint32_t nd_local = hb[1];
+  // the route and whether nodata occurs anywhere: one MAX all-reduce of {inexact, nodata occurs here}
+  DevBuf<int32_t> vote(2);
+  hb[0] = hb[0] != 0;
+  hb[1] = nd_local != NO_KEY;
+  RDB_CK(cudaMemcpyAsync(vote.p, hb, 2 * sizeof(int32_t), cudaMemcpyHostToDevice, c.stream));
+  comm_allreduce(comm, vote.p, 2, RDB200_MAX_I32);
+  RDB_CK(cudaMemcpyAsync(hb, vote.p, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  const bool rank_keys = hb[0] != 0, nd_found = hb[1] != 0;
+  if (ranked) *ranked = rank_keys;
+  if (inv) inv->ranked = rank_keys;
+  float nd;
+  if (!rank_keys) {  // cast route: (float)z in every band, no cap
+    nd = !nd_found ? nodata_image(nodata) : nd_local != NO_KEY ? host_bits_float(nd_local) : (float)nodata;
+    exchange_band_rows(comm, d_band_keys, sizeof(float), w, hloc, gt, gb);
+    return nd;
+  }
+
+  // rank route: local dense ranks and the band's sorted distinct values
+  RDB_CK(cudaMemsetAsync(d_distinct, 0, sizeof(uint32_t), c.stream));
+  DevBuf<double> table;
+  rank_route(d_z, d_key, n, nodata, &table, d_nd, d_distinct, d_hist);
+  DevBuf<long long> info(3);
+  band_table_bounds_kernel<<<1, 1, 0, c.stream>>>(table.p, d_distinct, nodata, info.p);
+  RDB_CK(cudaGetLastError());
+  count_launch();
+  long long hi[3];
+  RDB_CK(cudaMemcpyAsync(c.pinned, info.p, sizeof hi, cudaMemcpyDeviceToHost, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  memcpy(hi, c.pinned, sizeof hi);
+  const uint32_t lo = (uint32_t)hi[0];
+  const size_t m = (size_t)hi[1];
+
+  // every band's |D_b| (slot b) and sum_b |{u in D_b : u < nodata}| = r(nodata) (slot G): one SUM all-reduce, so every
+  // rank sees the same counts and takes the same decision on the cap
+  std::vector<int32_t> counts(world + 1, 0);
+  counts[rank] = (int32_t)m;
+  counts[world] = (int32_t)hi[2];
+  DevBuf<int32_t> d_counts(world + 1);
+  RDB_CK(cudaMemcpyAsync(d_counts.p, counts.data(), counts.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c.stream));
+  comm_allreduce(comm, d_counts.p, counts.size(), RDB200_SUM_I32);
+  RDB_CK(cudaMemcpyAsync(counts.data(), d_counts.p, counts.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, c.stream));
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  int64_t total = 0;
+  size_t maxm = 0;
+  for (int b = 0; b < world; b++) {
+    total += counts[b];
+    maxm = (size_t)counts[b] > maxm ? (size_t)counts[b] : maxm;
+  }
+  const int64_t cap = c.params.f64_band_rank_cap > 0 ? c.params.f64_band_rank_cap : ((int64_t)1 << 31) - ((int64_t)1 << 25);
+  if (total >= cap)
+    fail("float64 row bands: the bands hold %lld distinct values in all; order keys take fewer than %lld", (long long)total,
+         (long long)cap);
+
+  // the own message: [count | D_b], and r = the own term (the local dense rank) to which the chain adds the others
+  DevBuf<double> own(maxm + 1);
+  RDB_CK(cudaMemcpyAsync(own.p + 1, table.p + lo, m * sizeof(double), cudaMemcpyDeviceToDevice, c.stream));
+  table.reset();
+  set_msg_count(own.p, m);
+  DevBuf<uint32_t> r(m);
+  if (m) {  // (a band of NaN, +-inf and +-DBL_MAX only has no D_b)
+    iota_kernel<<<stream_blocks(m), 256, 0, c.stream>>>(r.p, m);
+    RDB_CK(cudaGetLastError());
+    count_launch();
+  }
+  const unsigned blocks = (unsigned)((m + maxm + MERGE_TILE - 1) / MERGE_TILE);
+  chain_pass(comm, own.p, maxm, [&](const double *msg) {
+    if (m == 0) return;
+    merge_count_kernel<<<blocks, 256, 0, c.stream>>>(own.p + 1, m, msg, r.p);
+    RDB_CK(cudaGetLastError());
+    count_launch();
+  });
+  band_gather_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_key, n, r.p, lo);
+  RDB_CK(cudaGetLastError());
+  count_launch();
+  const float img = sentinel_image(nodata);
+  nd = !nd_found ? nodata_image(nodata) : img != 0.f ? img : host_bits_float(RANK_BASE + (uint32_t)counts[world]);
+  exchange_band_rows(comm, d_band_keys, sizeof(float), w, hloc, gt, gb);
+  if (inv) {
+    inv->m = m;
+    inv->cap = maxm;
+    inv->vals.alloc(maxm + 1);
+    RDB_CK(cudaMemcpyAsync(inv->vals.p, own.p, (m + 1) * sizeof(double), cudaMemcpyDeviceToDevice, c.stream));
+    inv->keys.alloc(m);
+    RDB_CK(cudaMemcpyAsync(inv->keys.p, r.p, m * sizeof(uint32_t), cudaMemcpyDeviceToDevice, c.stream));
+  }
+  return nd;
+}
+
+// kappa_G^-1 of a filled key band into the owned rows of the double band: unraised cells keep their bits, raised cells
+// take the value of their key -- from the band's own table, else from the tables of the other bands.  The second chain
+// pass forwards (value, key) tables rather than the missing keys: a query pass would carry 12 B per distinct missing
+// level as a table carries 12 B per distinct value, and a band can miss as many levels as it owns cells, but the queries
+// would first have to be made distinct (a sort with its scratch).  The pass runs only when some band missed a level.
+void mgpu_f64_writeback_dev(const rdb200_comm *comm, const BandKeys &inv, double *d_band, const float *k0, const float *kf, int w,
+                            int hloc, int gt, int gb) {
+  Ctx &c = ctx();
+  gt = gt ? 1 : 0;
+  gb = gb ? 1 : 0;
+  const size_t n = (size_t)w * (hloc - gt - gb), off = (size_t)w * gt;
+  double *d_z = d_band + off;
+  k0 += off;
+  kf += off;
+  if (!inv.ranked) {
+    f64_writeback_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, k0, kf, n, nullptr);
+    RDB_CK(cudaGetLastError());
+    count_launch();
+    return;
+  }
+  DevBuf<uint8_t> pending(n);
+  DevBuf<int32_t> flag(2);  // [0] some level missed (MAX over the ranks), [1] some level still missing after the pass
+  RDB_CK(cudaMemsetAsync(flag.p, 0, 2 * sizeof(int32_t), c.stream));
+  band_writeback_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, k0, kf, n, inv.keys.p, inv.vals.p + 1, inv.m, pending.p,
+                                                                flag.p);
+  RDB_CK(cudaGetLastError());
+  count_launch();
+  comm_allreduce(comm, flag.p, 1, RDB200_MAX_I32);
+  if (read_i32(flag.p) == 0) return;
+  // the own table: [count | values (cap slots) | keys (cap uint32, in cap / 2 + 1 slots)]
+  const size_t cap = inv.cap, slots = cap + cap / 2 + 1;
+  DevBuf<double> own(slots + 1);
+  RDB_CK(cudaMemcpyAsync(own.p, inv.vals.p, (inv.m + 1) * sizeof(double), cudaMemcpyDeviceToDevice, c.stream));
+  RDB_CK(cudaMemcpyAsync(own.p + 1 + cap, inv.keys.p, inv.m * sizeof(uint32_t), cudaMemcpyDeviceToDevice, c.stream));
+  chain_pass(comm, own.p, slots, [&](const double *msg) {
+    band_lookup_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, kf, n, pending.p, msg, cap, nullptr);
+    RDB_CK(cudaGetLastError());
+    count_launch();
+  });
+  // every raised key is the key of some cell of the raster: a level found nowhere is a broken invariant
+  band_lookup_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, kf, n, pending.p, own.p, cap, flag.p + 1);
+  RDB_CK(cudaGetLastError());
+  count_launch();
+  if (read_i32(flag.p + 1)) fail("float64 row bands: a filled level has no value in any band");
+}
+
+// ResolveFlatsEpsilon's increment mask applied as double ulps (interior cells of the w x h raster only)
+void f64_apply_ulps_dev(double *d_z, const int32_t *d_mask, int w, int h) {
+  f64_apply_ulps_kernel<<<stream_blocks((size_t)w * h), 256, 0, ctx().stream>>>(d_z, d_mask, w, h);
+  RDB_CK(cudaGetLastError());
+  count_launch();
 }
 
 }  // namespace rdb

@@ -1116,18 +1116,19 @@ int flats_band_steps(const rdb200_comm *comm, rdb200_flats_state *s, bool from_d
 
 // ResolveFlatsEpsilon over row bands, driven from C++ over a rdb200_comm.  On return the ghost rows of d_local hold the
 // neighbours' resolved edge rows (one last exchange), so that accumulation can follow without another one.
-// *seam_iters: flag + height merge iterations (0 for one band).
+// *seam_iters: flag + height merge iterations (0 for one band).  With d_mask_out the increment mask goes there instead
+// (the float64 bands apply it as double ulps) and d_local is not modified.
 void mgpu_resolve_flats_band(const rdb200_comm *comm, float *d_local, int w, int hloc, float nodata, int gt, int gb,
-                             int *seam_iters) {
+                             int *seam_iters, int32_t *d_mask_out) {
   Ctx &c = ctx();
   check_band_args("mgpu_resolve_flats", comm, d_local, w, hloc, gt, gb);
   gt = gt ? 1 : 0;
   gb = gb ? 1 : 0;
   std::unique_ptr<rdb200_flats_state> s(flats_begin(d_local, w, hloc, nodata, gt, gb));
   const int iters = flats_band_steps(comm, s.get(), false);
-  flats_apply(s.get());
+  flats_apply(s.get(), d_mask_out);
   s.reset();
-  exchange_band_rows(comm, d_local, sizeof(float), w, hloc, gt, gb);  // the neighbours' resolved edge rows
+  if (!d_mask_out) exchange_band_rows(comm, d_local, sizeof(float), w, hloc, gt, gb);  // the neighbours' resolved edge rows
   RDB_CK(cudaStreamSynchronize(c.stream));
   if (seam_iters) *seam_iters = iters;
 }

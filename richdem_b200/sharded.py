@@ -305,6 +305,11 @@ def fill_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, solver_cls=None
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     import os
     cxx = solver_cls is None and os.environ.get("RDB_BAND_DRIVER", "cxx") != "python"
+    if _is_f64(local_dem):
+        if not cxx:
+            raise ValueError("fill_band: float64 bands run in the C++ band driver only; the Python band protocol "
+                             "(solver_cls, RDB_BAND_DRIVER=python) takes float32")
+        return _fill_band_f64(local_dem, g_top, g_bot, group, return_stats, row0, height, topology)
     if topology == "D4" and not cxx:
         raise ValueError("fill_band(topology='D4') runs in the C++ band driver only; the Python band protocol "
                          "(solver_cls, RDB_BAND_DRIVER=python) fills with D8")
@@ -368,10 +373,12 @@ def pit_mask_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: flo
     """PitMask over this rank's band.  ``local_dem`` is (g_top + owned + g_bot) x W; it is not modified and its ghost rows
     are not read.  ``row0`` / ``height`` as in :func:`fill_band` (gathered from the ranks when ``height`` <= 0).
     Collective.  Returns the uint8 mask of the local shape whose owned rows are the single-GPU bits (ghost rows
-    unspecified)."""
+    unspecified).  A float64 band gives the bits of :func:`richdem_b200.f64` on the whole raster."""
     from . import _lib
     if topology not in ("D8", "D4"):
         raise Exception("Unknown topology!")
+    if _is_f64(local_dem):
+        return _pit_mask_band_f64(local_dem, g_top, g_bot, nodata, topology, row0, height, group)
     assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
     row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
     _lib.use_torch_stream()
@@ -387,10 +394,12 @@ def has_depressions_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, topo
                          height: int = 0, group=None) -> bool:
     """HasDepressions of the whole raster, from this rank's band (arguments as :func:`pit_mask_band`).  A strict pit in any
     band answers after one all-reduce; the band fill runs only when there is none.  Collective; every rank gets the
-    same answer."""
+    same answer.  Float64 bands too."""
     from . import _lib
     if topology not in ("D8", "D4"):
         raise Exception("Unknown topology!")
+    if _is_f64(local_dem):
+        return _has_depressions_band_f64(local_dem, g_top, g_bot, topology, row0, height, group)
     assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
     row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
     _lib.use_torch_stream()
@@ -544,11 +553,17 @@ def fa_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: float, di
     otherwise call :func:`exchange_rows`).  ``weights`` (float64, same local shape) defaults to ones.
     ``method`` / ``exponent`` as in :func:`richdem_b200.FlowAccumulation` (D8, Dinf, D4, Quinn, Holmgren, Freeman and
     their aliases); without a method, ``dinf`` picks FA_Tarboton or FA_D8.
-    Returns (local accumulation incl. scratch ghost rows, exchange rounds[, stats])."""
+    Returns (local accumulation incl. scratch ghost rows, exchange rounds[, stats]).  A float64 ``local_dem`` runs
+    rdb200_mgpu_fa_method_f64_f64, which does not read its ghost rows."""
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     mid, xparam = fa_method_id(method, exponent, dinf)
     import os
+    if _is_f64(local_dem):
+        if accumulator_cls is not None or os.environ.get("RDB_BAND_DRIVER", "cxx") == "python":
+            raise ValueError("fa_band: float64 bands run in the C++ band driver only; the Python band protocol "
+                             "(accumulator_cls, RDB_BAND_DRIVER=python) takes float32")
+        return _fa_band_f64(local_dem, g_top, g_bot, nodata, weights, group, return_stats, mid, xparam)
     if accumulator_cls is None and os.environ.get("RDB_BAND_DRIVER", "cxx") != "python":
         from . import _lib
         ones = weights is None
@@ -803,8 +818,11 @@ def resolve_flats_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata
     ghost rows must hold the neighbours' elevation rows; on return they hold the neighbours' resolved
     edge rows, so :func:`fa_band` can follow without :func:`exchange_rows`).  Collective.  Returns the
     number of seam iterations (flags + heights).  The protocol runs in C++ over the library's
-    communicator (csrc/flats.cu: mgpu_resolve_flats_band)."""
+    communicator (csrc/flats.cu: mgpu_resolve_flats_band).  A float64 band takes its increments as double ulps and
+    its ghost rows are not read on entry."""
     from . import _lib
+    if _is_f64(local_dem):
+        return _resolve_flats_band_f64(local_dem, g_top, g_bot, nodata, group)
     assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
     _lib.use_torch_stream()
     h, w = local_dem.shape
@@ -864,6 +882,8 @@ def flow_proportions_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nod
     rows are the single-GPU bits (ghost rows scratch)."""
     from . import _lib
     mid, xparam = _method_id(method, exponent, "FlowProportions")
+    if _is_f64(local_dem):
+        return _flow_proportions_band_f64(local_dem, g_top, g_bot, nodata, mid, xparam, group)
     assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
     _lib.use_torch_stream()
     h, w = local_dem.shape
@@ -908,6 +928,8 @@ def terrain_attribute_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, at
     float32 attribute of the local shape, NoData -9999, whose owned rows are the single-GPU bits (ghost rows scratch)."""
     from . import _lib, _terrain_attrib_id
     aid = _terrain_attrib_id(attrib)
+    if _is_f64(local_dem):
+        return _terrain_attribute_band_f64(local_dem, g_top, g_bot, aid, nodata, zscale, cell_x, cell_y, group)
     assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
     _lib.use_torch_stream()
     h, w = local_dem.shape
@@ -917,3 +939,112 @@ def terrain_attribute_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, at
                                                             float(nodata), -9999.0, float(zscale), float(cell_x), float(cell_y),
                                                             int(g_top), int(g_bot)))
     return out
+
+
+# =================================================================================================
+# float64 bands: the C++ band drivers on float keys every band shares (csrc/f64.cu: kappa_G), and the double flow
+# metrics and attributes (csrc/f64_band.cu).  NoData is a double.
+# =================================================================================================
+def _is_f64(t) -> bool:
+    return torch is not None and isinstance(t, torch.Tensor) and t.dtype == torch.float64
+
+
+def _f64_band(local_dem):
+    from . import _lib
+    assert _on_device(local_dem) and local_dem.dtype == torch.float64 and local_dem.is_contiguous()
+    _lib.use_torch_stream()
+    return _lib, _lib.lib()
+
+
+def _fill_band_f64(local_dem, g_top, g_bot, group, return_stats, row0, height, topology):
+    _lib, L = _f64_band(local_dem)
+    row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
+    h, w = local_dem.shape
+    xr = C.c_int32(0)
+    cm = lib_comm(group, local_dem.is_cuda)
+    fn = L.rdb200_mgpu_fill_depressions_d8_f64 if topology == "D8" else L.rdb200_mgpu_fill_depressions_d4_f64
+    _lib.check(fn(cm.handle, local_dem.data_ptr(), w, h, int(g_top), int(g_bot), row0, height, C.byref(xr)))
+    if return_stats:
+        return local_dem, int(xr.value), _lib.stats()
+    return local_dem, int(xr.value)
+
+
+def _pit_mask_band_f64(local_dem, g_top, g_bot, nodata, topology, row0, height, group):
+    _lib, L = _f64_band(local_dem)
+    row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
+    h, w = local_dem.shape
+    mask = torch.empty((h, w), dtype=torch.uint8, device=local_dem.device)
+    cm = lib_comm(group, local_dem.is_cuda)
+    fn = L.rdb200_mgpu_pit_mask_d8_f64 if topology == "D8" else L.rdb200_mgpu_pit_mask_d4_f64
+    _lib.check(fn(cm.handle, local_dem.data_ptr(), mask.data_ptr(), w, h, float(nodata), int(g_top), int(g_bot), row0, height))
+    return mask
+
+
+def _has_depressions_band_f64(local_dem, g_top, g_bot, topology, row0, height, group):
+    _lib, L = _f64_band(local_dem)
+    row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
+    h, w = local_dem.shape
+    out = C.c_int32(0)
+    cm = lib_comm(group, local_dem.is_cuda)
+    fn = L.rdb200_mgpu_has_depressions_d8_f64 if topology == "D8" else L.rdb200_mgpu_has_depressions_d4_f64
+    _lib.check(fn(cm.handle, local_dem.data_ptr(), w, h, int(g_top), int(g_bot), row0, height, C.byref(out)))
+    return bool(out.value)
+
+
+def _resolve_flats_band_f64(local_dem, g_top, g_bot, nodata, group):
+    _lib, L = _f64_band(local_dem)
+    h, w = local_dem.shape
+    it = C.c_int32(0)
+    cm = lib_comm(group, local_dem.is_cuda)
+    _lib.check(L.rdb200_mgpu_resolve_flats_epsilon_f64(cm.handle, local_dem.data_ptr(), w, h, float(nodata), int(g_top),
+                                                       int(g_bot), C.byref(it)))
+    return int(it.value)
+
+
+def _fa_band_f64(local_dem, g_top, g_bot, nodata, weights, group, return_stats, mid, xparam):
+    _lib, L = _f64_band(local_dem)
+    ones = weights is None
+    acc = torch.empty(local_dem.shape, dtype=torch.float64, device=local_dem.device) if ones else weights
+    assert _on_device(acc) and acc.dtype == torch.float64 and acc.is_contiguous()
+    xr = C.c_int32(0)
+    cm = lib_comm(group, local_dem.is_cuda)
+    _lib.check(L.rdb200_mgpu_fa_method_f64_f64(cm.handle, local_dem.data_ptr(), acc.data_ptr(), local_dem.shape[1],
+                                               local_dem.shape[0], float(nodata), int(g_top), int(g_bot), mid, xparam, int(ones),
+                                               C.byref(xr)))
+    if return_stats:
+        return acc, int(xr.value), _lib.stats()
+    return acc, int(xr.value)
+
+
+def _flow_proportions_band_f64(local_dem, g_top, g_bot, nodata, mid, xparam, group):
+    _lib, L = _f64_band(local_dem)
+    h, w = local_dem.shape
+    props = torch.empty((h, w, 9), dtype=torch.float32, device=local_dem.device)
+    cm = lib_comm(group, local_dem.is_cuda)
+    _lib.check(L.rdb200_mgpu_fm_method_f64(cm.handle, mid, local_dem.data_ptr(), props.data_ptr(), w, h, float(nodata),
+                                           int(g_top), int(g_bot), xparam))
+    return props
+
+
+def _terrain_attribute_band_f64(local_dem, g_top, g_bot, aid, nodata, zscale, cell_x, cell_y, group):
+    _lib, L = _f64_band(local_dem)
+    h, w = local_dem.shape
+    out = torch.empty((h, w), dtype=torch.float32, device=local_dem.device)
+    cm = lib_comm(group, local_dem.is_cuda)
+    _lib.check(L.rdb200_mgpu_terrain_attribute_f64(cm.handle, aid, local_dem.data_ptr(), out.data_ptr(), w, h, float(nodata),
+                                                   -9999.0, float(zscale), float(cell_x), float(cell_y), int(g_top), int(g_bot)))
+    return out
+
+
+def f64_order_keys_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: float, group=None):
+    """Diagnostic (not a stable interface): kappa_G, the float keys the float64 band drivers run the float32 engines on.
+    Collective.  Returns (float32 keys of the local shape, whose ghost rows hold the neighbours' keys, kappa_G(nodata),
+    True for global ranks / False for the cast to float)."""
+    _lib, L = _f64_band(local_dem)
+    h, w = local_dem.shape
+    keys = torch.empty((h, w), dtype=torch.float32, device=local_dem.device)
+    nd, ranked = C.c_float(0), C.c_int32(0)
+    cm = lib_comm(group, local_dem.is_cuda)
+    _lib.check(L.rdb200_mgpu_f64_order_keys(cm.handle, local_dem.data_ptr(), keys.data_ptr(), w, h, float(nodata), int(g_top),
+                                            int(g_bot), C.byref(nd), C.byref(ranked)))
+    return keys, float(nd.value), bool(ranked.value)
