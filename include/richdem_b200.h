@@ -203,6 +203,18 @@ RDB200_API int rdb200_d8_flow_directions_f64(const double *dem, uint8_t *flowdir
                                              double nodata);
 RDB200_API int rdb200_fa_d8_f64_f64(const double *dem, double *accum_inout, int32_t width, int32_t height, double nodata,
                                     int32_t accum_is_ones);
+/* GetFlatMask<double> (flats/Barnes2014.hpp:398-467) as rdb200_get_flat_mask_f32: the mask bit for bit, the labels equal
+ * to the reference's as a partition of the cells. */
+RDB200_API int rdb200_get_flat_mask_f64(const double *dem, int32_t *flat_mask, int32_t *labels, int32_t width, int32_t height,
+                                        double nodata);
+/* barnes_flat_resolution_d8<double, uint8_t> (flats/flat_resolution.hpp:588-607) as rdb200_d8_flow_directions_flats_f32:
+ * directions of the doubles, the flats of that direction grid resolved on the keys, then d8_flow_flats, or with alter != 0
+ * d8_flats_alter_dem and the directions of the altered doubles.  The reference alters a double with nextafterf
+ * (:565-568): a labelled interior cell with increment count m > 0 becomes the double of m float-ulp steps towards +inf
+ * from the double rounded to the nearest float (so +inf from any double above FLT_MAX), m = 0 leaves it as it is.  The
+ * directions and the altered dem are bit-identical. */
+RDB200_API int rdb200_d8_flow_directions_flats_f64(double *dem, uint8_t *flowdirs, int32_t width, int32_t height, double nodata,
+                                                   int32_t alter);
 RDB200_API int rdb200_fa_d4_f64_f64(const double *dem, double *accum_inout, int32_t width, int32_t height, double nodata);
 /* DIAGNOSTIC, not part of the stable interface: the key encoding is an implementation detail of the entry points above
  * and may change between versions (tests use these two to check it).  kappa itself: keys (width x height floats), *nodata_key = kappa(nodata) (the key of a cell equal to nodata; else the
@@ -328,6 +340,8 @@ RDB200_API int rdb200_dev_has_depressions_d4_f64(const double *d_dem, int32_t wi
 RDB200_API int rdb200_dev_resolve_flats_epsilon_f64(double *d_dem, int32_t width, int32_t height, double nodata);
 RDB200_API int rdb200_dev_d8_flow_directions_f64(const double *d_dem, uint8_t *d_flowdirs, int32_t width, int32_t height,
                                                  double nodata);
+RDB200_API int rdb200_dev_d8_flow_directions_flats_f64(double *d_dem, uint8_t *d_flowdirs, int32_t width, int32_t height,
+                                                       double nodata, int32_t alter);
 RDB200_API int rdb200_dev_fa_d8_f64_f64(const double *d_dem, double *d_accum_inout, int32_t width, int32_t height,
                                         double nodata, int32_t accum_is_ones);
 RDB200_API int rdb200_dev_fa_d4_f64_f64(const double *d_dem, double *d_accum_inout, int32_t width, int32_t height,
@@ -505,7 +519,10 @@ RDB200_API int rdb200_mgpu_flow_accumulation_props_f64(const rdb200_comm *comm, 
  *   pit_mask_*_f64, has_depressions_*_f64   d_band not modified, its ghost rows not read
  *   resolve_flats_epsilon_f64  ghost rows not read on entry, the neighbours' resolved edge rows on return
  *   fm_method_f64, terrain_attribute_f64   ghost rows of d_band_dem refreshed, as the float32 calls do
- *   fa_method_f64_f64          methods as rdb200_mgpu_fa_method_f32_f64; ghost rows of d_band_dem not read */
+ *   fa_method_f64_f64          methods as rdb200_mgpu_fa_method_f32_f64; ghost rows of d_band_dem not read
+ *   d8_flow_directions_flats_f64  as rdb200_mgpu_d8_flow_directions_flats_f32: the ghost rows of d_band_dem hold the
+ *                              neighbours' edge rows on entry; the directions of the doubles, the flats on kappa_G, and
+ *                              with alter = 1 the float steps of rdb200_d8_flow_directions_flats_f64 on the owned rows */
 RDB200_API int rdb200_mgpu_fill_depressions_d8_f64(const rdb200_comm *comm, double *d_band, int32_t width, int32_t local_rows,
                                                    int32_t ghost_top, int32_t ghost_bottom, int32_t row0, int32_t height,
                                                    int32_t *exchange_rounds);
@@ -527,6 +544,9 @@ RDB200_API int rdb200_mgpu_has_depressions_d4_f64(const rdb200_comm *comm, const
 RDB200_API int rdb200_mgpu_resolve_flats_epsilon_f64(const rdb200_comm *comm, double *d_band, int32_t width, int32_t local_rows,
                                                      double nodata, int32_t ghost_top, int32_t ghost_bottom,
                                                      int32_t *seam_iterations);
+RDB200_API int rdb200_mgpu_d8_flow_directions_flats_f64(const rdb200_comm *comm, double *d_band_dem, uint8_t *d_band_dirs,
+                                                        int32_t width, int32_t local_rows, double nodata, int32_t ghost_top,
+                                                        int32_t ghost_bottom, int32_t alter, int32_t *seam_iterations);
 RDB200_API int rdb200_mgpu_fm_method_f64(const rdb200_comm *comm, int32_t method, double *d_band_dem, float *d_band_props9,
                                          int32_t width, int32_t local_rows, double nodata, int32_t ghost_top, int32_t ghost_bottom,
                                          double xparam);

@@ -411,6 +411,15 @@ inline void d8_flow_directions<double, uint8_t>(const Array2D<double> &elevation
   richdem_b200::check(rdb200_d8_flow_directions_f64(elevations.data(), flowdirs.data(), elevations.width(),
                                                     elevations.height(), elevations.noData()));
 }
+// flats/flat_resolution.hpp:588-607; with alter the doubles take the reference's nextafterf steps
+template <>
+inline void barnes_flat_resolution_d8<double, uint8_t>(Array2D<double> &elevations, Array2D<uint8_t> &flowdirs, bool alter) {
+  flowdirs.resize(elevations);
+  flowdirs.setNoData(FLOWDIR_NO_DATA);
+  richdem_b200::check(rdb200_d8_flow_directions_flats_f64(elevations.data(), flowdirs.data(), elevations.width(),
+                                                          elevations.height(), elevations.noData(), alter ? 1 : 0));
+  flowdirs.templateCopy(elevations);
+}
 // methods/flow_accumulation.hpp:27,28; accum holds the weights, as for float
 template <>
 inline void FA_D8<double, double>(const Array2D<double> &elevations, Array2D<double> &accum) {

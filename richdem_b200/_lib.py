@@ -96,6 +96,9 @@ SIGNATURES = {
     "rdb200_has_depressions_d4_f64": [_vp, _i32, _i32, C.POINTER(_i32)],
     "rdb200_resolve_flats_epsilon_f64": [_vp, _i32, _i32, _f64],
     "rdb200_d8_flow_directions_f64": [_vp, _vp, _i32, _i32, _f64],
+    "rdb200_get_flat_mask_f64": [_vp, _vp, _vp, _i32, _i32, _f64],
+    "rdb200_d8_flow_directions_flats_f64": [_vp, _vp, _i32, _i32, _f64, _i32],
+    "rdb200_dev_d8_flow_directions_flats_f64": [_vp, _vp, _i32, _i32, _f64, _i32],
     "rdb200_fa_d8_f64_f64": [_vp, _vp, _i32, _i32, _f64, _i32],
     "rdb200_fa_d4_f64_f64": [_vp, _vp, _i32, _i32, _f64],
     "rdb200_f64_order_keys": [_vp, _vp, _i32, _i32, _f64, C.POINTER(_f32), C.POINTER(_i32)],
@@ -147,6 +150,7 @@ SIGNATURES = {
     "rdb200_mgpu_has_depressions_d8_f64": [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
     "rdb200_mgpu_has_depressions_d4_f64": [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, C.POINTER(_i32)],
     "rdb200_mgpu_resolve_flats_epsilon_f64": [_vp, _vp, _i32, _i32, _f64, _i32, _i32, C.POINTER(_i32)],
+    "rdb200_mgpu_d8_flow_directions_flats_f64": [_vp, _vp, _vp, _i32, _i32, _f64, _i32, _i32, _i32, C.POINTER(_i32)],
     "rdb200_mgpu_fm_method_f64": [_vp, _i32, _vp, _vp, _i32, _i32, _f64, _i32, _i32, _f64],
     "rdb200_mgpu_terrain_attribute_f64": [_vp, _i32, _vp, _vp, _i32, _i32, _f64, _f32, _f32, _f64, _f64, _i32, _i32],
     "rdb200_mgpu_fa_method_f64_f64": [_vp, _vp, _vp, _i32, _i32, _f64, _i32, _i32, _i32, _f64, _i32, C.POINTER(_i32)],

@@ -364,6 +364,21 @@ static int d8_flow_directions_f64(Side side, const double *dem, uint8_t *dirs, i
                      [&](Arrays &a, size_t n) { d8_flow_directions_f64_dev(a.in(dem, n), a.out(dirs, n), w, h, nodata); });
 }
 
+// reference flats/Barnes2014.hpp:398-467 (GetFlatMask, T = double)
+static int get_flat_mask_f64(Side side, const double *dem, int32_t *flat_mask, int32_t *labels, int32_t w, int32_t h,
+                             double nodata) {
+  return raster_call(side, "get_flat_mask: null pointer", {dem, flat_mask, labels}, w, h, [&](Arrays &a, size_t n) {
+    get_flat_mask_f64_dev(a.in(dem, n), a.out(flat_mask, n), a.out(labels, n), w, h, nodata);
+  });
+}
+
+// reference flats/flat_resolution.hpp:588-607 (barnes_flat_resolution_d8<double, uint8_t>); dem is written only with alter
+static int d8_flow_directions_flats_f64(Side side, double *dem, uint8_t *dirs, int32_t w, int32_t h, double nodata, int32_t alter) {
+  return raster_call(side, "d8_flow_directions_flats: null pointer", {dem, dirs}, w, h, [&](Arrays &a, size_t n) {
+    d8_flow_directions_flats_f64_dev(alter ? a.inout(dem, n) : a.in(dem, n), a.out(dirs, n), w, h, nodata, alter != 0);
+  });
+}
+
 // reference methods/flow_accumulation.hpp:27 (FA_D8<double, double>: OCallaghan1984.hpp:13-91 + flow_accumulation_generic.hpp:33-100)
 static int fa_d8_f64(Side side, const double *dem, double *accum, int32_t w, int32_t h, double nodata, int32_t ones) {
   return raster_call(side, "flow accumulation: null pointer", {dem, accum}, w, h, [&](Arrays &a, size_t n) {
@@ -696,6 +711,12 @@ int rdb200_resolve_flats_epsilon_f64(double *dem, int32_t w, int32_t h, double n
 int rdb200_d8_flow_directions_f64(const double *dem, uint8_t *dirs, int32_t w, int32_t h, double nodata) {
   return d8_flow_directions_f64(Side::host, dem, dirs, w, h, nodata);
 }
+int rdb200_get_flat_mask_f64(const double *dem, int32_t *flat_mask, int32_t *labels, int32_t w, int32_t h, double nodata) {
+  return get_flat_mask_f64(Side::host, dem, flat_mask, labels, w, h, nodata);
+}
+int rdb200_d8_flow_directions_flats_f64(double *dem, uint8_t *dirs, int32_t w, int32_t h, double nodata, int32_t alter) {
+  return d8_flow_directions_flats_f64(Side::host, dem, dirs, w, h, nodata, alter);
+}
 int rdb200_fa_d8_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata, int32_t ones) {
   return fa_d8_f64(Side::host, dem, accum, w, h, nodata, ones);
 }
@@ -824,6 +845,9 @@ int rdb200_dev_resolve_flats_epsilon_f64(double *d_dem, int32_t w, int32_t h, do
 }
 int rdb200_dev_d8_flow_directions_f64(const double *d_dem, uint8_t *d_dirs, int32_t w, int32_t h, double nodata) {
   return d8_flow_directions_f64(Side::device, d_dem, d_dirs, w, h, nodata);
+}
+int rdb200_dev_d8_flow_directions_flats_f64(double *d_dem, uint8_t *d_dirs, int32_t w, int32_t h, double nodata, int32_t alter) {
+  return d8_flow_directions_flats_f64(Side::device, d_dem, d_dirs, w, h, nodata, alter);
 }
 int rdb200_dev_fa_d8_f64_f64(const double *d_dem, double *d_accum, int32_t w, int32_t h, double nodata, int32_t ones) {
   return fa_d8_f64(Side::device, d_dem, d_accum, w, h, nodata, ones);
@@ -1009,6 +1033,19 @@ int rdb200_mgpu_resolve_flats_epsilon_f64(const rdb200_comm *comm, double *d_ban
   int it = 0;
   const int rc = raster_call(Side::device, "mgpu_resolve_flats: null pointer", {comm, d_band}, w, rows,
                              [&](Arrays &, size_t) { mgpu_resolve_flats_f64_band(comm, d_band, w, rows, nodata, gt, gb, &it); });
+  if (rc == 0 && seam_iterations) *seam_iterations = it;
+  return rc;
+}
+
+int rdb200_mgpu_d8_flow_directions_flats_f64(const rdb200_comm *comm, double *d_band_dem, uint8_t *d_band_dirs, int32_t w,
+                                             int32_t rows, double nodata, int32_t gt, int32_t gb, int32_t alter,
+                                             int32_t *seam_iterations) {
+  int it = 0;
+  const int rc = raster_call(Side::device, "mgpu_d8_flow_directions_flats: null pointer", {comm, d_band_dem, d_band_dirs}, w, rows,
+                             [&](Arrays &, size_t) {
+                               mgpu_d8_flow_directions_flats_f64_band(comm, d_band_dem, d_band_dirs, w, rows, nodata, gt, gb,
+                                                                      alter != 0, &it);
+                             });
   if (rc == 0 && seam_iterations) *seam_iterations = it;
   return rc;
 }

@@ -197,6 +197,10 @@ void mgpu_resolve_flats_band(const rdb200_comm *comm, float *d_local, int w, int
                              int *seam_iters, int32_t *d_mask_out = nullptr);
 void mgpu_d8_flow_directions_flats_band(const rdb200_comm *comm, float *d_dem, uint8_t *d_dirs, int w, int hloc, float nodata,
                                         int gt, int gb, bool alter, int *seam_iters);
+// the flats of a band's plain D8 directions resolved over the bands (barnes_flat_resolution_d8 between its two direction
+// passes); with alter, d_mask_out (may be null) receives the increment mask instead of d_dem its float ulps
+int mgpu_dir_flats_band(const rdb200_comm *comm, float *d_dem, uint8_t *d_dirs, int w, int hloc, float nodata, int gt, int gb,
+                        bool alter, int32_t *d_mask_out);
 void mgpu_d8_flow_accum_band(const rdb200_comm *comm, const uint8_t *d_dirs, int32_t *d_area, int w, int hloc, int gt, int gb,
                              int *xrounds);
 // the band relaxation protocol over a state that holds its start; R sweep rounds between halo exchanges (0: none)
@@ -213,6 +217,8 @@ void resolve_flats_dev(float *d_dem, int w, int h, float nodata, int32_t *d_mask
                        int32_t *d_labels_out, bool apply, const uint8_t *d_dirs = nullptr);
 void d8_flow_directions_flats_dev(float *d_dem, uint8_t *d_dirs, int w, int h, float nodata, bool alter);
 void d8_flow_directions_dev(const float *d_dem, uint8_t *d_dirs, int w, int h, float nodata);
+// d8_flow_flats: interior NO_FLOW cells take the direction of their lowest same-label neighbour in the increment mask
+void d8_flow_flats_dev(const int32_t *d_mask, const int32_t *d_labels, uint8_t *d_dirs, int w, int h);
 void d8_flow_accum_dev(const uint8_t *d_dirs, int32_t *d_area, int w, int h);
 void fm_d8_dev(const float *d_dem, float *d_props, int w, int h, float nodata);
 void fm_tarboton_dev(const float *d_dem, float *d_props, int w, int h, float nodata);
@@ -253,6 +259,10 @@ void fa_tarboton_f64_dev(const double *d_dem, double *d_accum, int w, int h, dou
 void terrain_attribute_f64_dev(int attribute_id, const double *d_dem, float *d_out, int w, int h, double nodata_in,
                                float nodata_out, float zscale, double cell_x, double cell_y);
 void f64_apply_ulps_dev(double *d_z, const int32_t *d_mask, int w, int h);
+// d8_flats_alter_dem on doubles: the reference's nextafterf, i.e. k float ulps of the double rounded to float
+void f64_float_steps_dev(double *d_z, const int32_t *d_mask, int w, int h);
+void get_flat_mask_f64_dev(const double *d_z, int32_t *d_mask, int32_t *d_labels, int w, int h, double nodata);
+void d8_flow_directions_flats_f64_dev(double *d_z, uint8_t *d_dirs, int w, int h, double nodata, bool alter);
 int32_t read_i32(const int32_t *d_value);  // one device int, read back after the library's stream
 
 // ---- float64 row bands: kappa_G, one key map shared by every band (f64.cu), and the band drivers (f64_band.cu) ----
@@ -281,6 +291,8 @@ bool mgpu_has_depressions_f64_band(const rdb200_comm *comm, const double *d_band
                                    bool topo4);
 void mgpu_resolve_flats_f64_band(const rdb200_comm *comm, double *d_band, int w, int hloc, double nodata, int gt, int gb,
                                  int *seam_iters);
+void mgpu_d8_flow_directions_flats_f64_band(const rdb200_comm *comm, double *d_band, uint8_t *d_dirs, int w, int hloc, double nodata,
+                                            int gt, int gb, bool alter, int *seam_iters);
 void mgpu_fa_f64_band(const rdb200_comm *comm, const double *d_dem, double *d_accum, int w, int hloc, double nodata, int gt, int gb,
                       int method, double xparam, bool ones, int *xrounds);
 

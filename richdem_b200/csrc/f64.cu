@@ -352,6 +352,79 @@ __global__ void __launch_bounds__(256) f64_apply_ulps_kernel(double *__restrict_
   }
 }
 
+// d8_flats_alter_dem's step on a double (flats/flat_resolution.hpp:565-568).  The reference calls nextafterf even for
+// U = double, so the double is rounded to the nearest float (ties to even, overflow to +-inf), takes k float-ulp steps
+// towards +inf that saturate at +inf, and the float is widened back.  Both conversions are integer arithmetic on the
+// bits, so subnormal doubles and floats take the IEEE path whatever flush-to-zero setting the build uses.  A NaN cell
+// never carries a flat label (it equals no neighbour); it is returned unchanged.
+__device__ __forceinline__ uint32_t f32_bits_rn(double z) {
+  const uint64_t b = (uint64_t)__double_as_longlong(z);
+  const uint32_t sign = (uint32_t)(b >> 32) & 0x80000000u;
+  const uint64_t mag = b & 0x7fffffffffffffffull;
+  const int fe = (int)(mag >> 52) - 1023 + 127;  // biased float exponent of a normal result
+  if (fe >= 255) return sign | 0x7f800000u;       // +-inf and every double from 2^128 up
+  uint32_t r;
+  uint64_t rem, half;
+  if (fe >= 1) {
+    r = ((uint32_t)fe << 23) | (uint32_t)((mag & 0x000fffffffffffffull) >> 29);
+    rem = mag & 0x1fffffffull;
+    half = 0x10000000ull;
+  } else {  // a float subnormal, in units of 2^-149; a carry out of the fraction gives FLT_MIN's encoding
+    const int shift = 30 - fe;
+    if (shift > 54) return sign;  // below half of the least subnormal (double subnormals included)
+    const uint64_t sig = (mag & 0x000fffffffffffffull) | 0x0010000000000000ull;
+    r = (uint32_t)(sig >> shift);
+    rem = sig & ((1ull << shift) - 1);
+    half = 1ull << (shift - 1);
+  }
+  if (rem > half || (rem == half && (r & 1u))) r++;  // a carry into the exponent is the right rounding, up to +inf
+  return sign | r;
+}
+
+__device__ __forceinline__ double f64_of_f32_bits(uint32_t f) {
+  const uint64_t sign = (uint64_t)(f & 0x80000000u) << 32;
+  const uint32_t mag = f & 0x7fffffffu;
+  if (mag >= 0x7f800000u) return __longlong_as_double((long long)(sign | 0x7ff0000000000000ull | ((uint64_t)(mag & 0x7fffffu) << 29)));
+  if (mag == 0) return __longlong_as_double((long long)sign);
+  int e = (int)(mag >> 23);
+  uint32_t m = mag & 0x7fffffu;
+  if (e == 0) {  // subnormal: normalise
+    e = 1;
+    while (!(m & 0x800000u)) {
+      m <<= 1;
+      e--;
+    }
+    m &= 0x7fffffu;
+  }
+  return __longlong_as_double((long long)(sign | ((uint64_t)(e - 127 + 1023) << 52) | ((uint64_t)m << 29)));
+}
+
+__device__ __forceinline__ double float_steps_f64(double z, int k) {
+  if (k <= 0 || z != z) return z;
+  const uint32_t f = f32_bits_rn(z);
+  const bool neg = (f >> 31) != 0;
+  const long long mag = (long long)(f & 0x7fffffffu);
+  long long key = (neg ? -mag : mag) + k;  // as flats.cu's advance_ulps: -0.0 and +0.0 share key 0
+  uint32_t r;
+  if (key >= 0x7f800000ll) r = 0x7f800000u;
+  else if (key > 0) r = (uint32_t)key;
+  else if (key == 0) r = neg ? 0x80000000u : 0u;
+  else r = 0x80000000u | (uint32_t)(-key);
+  return f64_of_f32_bits(r);
+}
+
+// d8_flats_alter_dem (flat_resolution.hpp:546-580) with the increment mask of the key raster: interior cells only
+__global__ void __launch_bounds__(256) f64_float_steps_kernel(double *__restrict__ z, const int32_t *__restrict__ mask, int W,
+                                                              int H) {
+  const size_t n = (size_t)W * H, stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int m = mask[i];
+    if (m <= 0) continue;
+    const int y = (int)(i / W), x = (int)(i - (size_t)y * W);
+    if (x > 0 && y > 0 && x < W - 1 && y < H - 1) z[i] = float_steps_f64(z[i], m);
+  }
+}
+
 unsigned stream_blocks(size_t n) {
   const size_t want = (n + 255) / 256, cap = (size_t)ctx().num_sms * 8;
   return (unsigned)(want < cap ? want : cap);
@@ -517,6 +590,35 @@ void resolve_flats_f64_dev(double *d_z, int w, int h, double nodata) {
   f64_apply_ulps_kernel<<<stream_blocks(n), 256, 0, c.stream>>>(d_z, mask.p, w, h);
   RDB_CK(cudaGetLastError());
   count_launch();
+}
+
+// GetFlatMask<double>: the increment mask and labels of the key raster (the flats compare elevations only)
+void get_flat_mask_f64_dev(const double *d_z, int32_t *d_mask, int32_t *d_labels, int w, int h, double nodata) {
+  const size_t n = (size_t)w * h;
+  DevBuf<float> key(n);
+  const float nd = f64_keys_dev(d_z, key.p, n, nodata, nullptr, nullptr);
+  resolve_flats_dev(key.p, w, h, nd, d_mask, d_labels, false);
+}
+
+// barnes_flat_resolution_d8<double, uint8_t> (flats/flat_resolution.hpp:588-607): D8 directions of the doubles, then the
+// increment mask and labels of the flats the direction grid shows, on the keys (flats_from_dirs_kernel compares with ==
+// and < only), then either d8_flow_flats or d8_flats_alter_dem's float steps on the doubles and their directions again
+void d8_flow_directions_flats_f64_dev(double *d_z, uint8_t *d_dirs, int w, int h, double nodata, bool alter) {
+  Ctx &c = ctx();
+  const size_t n = (size_t)w * h;
+  d8_flow_directions_f64_dev(d_z, d_dirs, w, h, nodata);
+  DevBuf<float> key(n);
+  const float nd = f64_keys_dev(d_z, key.p, n, nodata, nullptr, nullptr);
+  DevBuf<int32_t> mask(n), labels(alter ? 0 : n);
+  resolve_flats_dev(key.p, w, h, nd, mask.p, alter ? nullptr : labels.p, false, d_dirs);
+  key.reset();
+  if (alter) {
+    f64_float_steps_dev(d_z, mask.p, w, h);
+    d8_flow_directions_f64_dev(d_z, d_dirs, w, h, nodata);
+  } else {
+    d8_flow_flats_dev(mask.p, labels.p, d_dirs, w, h);
+  }
+  RDB_CK(cudaStreamSynchronize(c.stream));
 }
 
 // FA_D8 (unit or given weights) on the key raster: the accumulation carries no elevation values
@@ -904,6 +1006,13 @@ void mgpu_f64_writeback_dev(const rdb200_comm *comm, const BandKeys &inv, double
 // ResolveFlatsEpsilon's increment mask applied as double ulps (interior cells of the w x h raster only)
 void f64_apply_ulps_dev(double *d_z, const int32_t *d_mask, int w, int h) {
   f64_apply_ulps_kernel<<<stream_blocks((size_t)w * h), 256, 0, ctx().stream>>>(d_z, d_mask, w, h);
+  RDB_CK(cudaGetLastError());
+  count_launch();
+}
+
+// d8_flats_alter_dem's float steps of the increment mask (interior cells of the w x h raster only)
+void f64_float_steps_dev(double *d_z, const int32_t *d_mask, int w, int h) {
+  f64_float_steps_kernel<<<stream_blocks((size_t)w * h), 256, 0, ctx().stream>>>(d_z, d_mask, w, h);
   RDB_CK(cudaGetLastError());
   count_launch();
 }

@@ -97,6 +97,36 @@ void mgpu_resolve_flats_f64_band(const rdb200_comm *comm, double *d_band, int w,
   RDB_CK(cudaStreamSynchronize(c.stream));
 }
 
+// barnes_flat_resolution_d8<double> over row bands: the plain directions come from the doubles (their ghost rows hold the
+// neighbours' edge rows on entry, as the band fill leaves them), the flats of those directions are resolved by the
+// float32 band protocol on kappa_G, and then either d8_flow_flats (alter = 0) or the float steps of d8_flats_alter_dem on
+// the owned rows, one exchange of the altered edge rows and the directions of the doubles again (alter = 1).  On return
+// the ghost rows of d_dirs (and, with alter = 1, of d_band) hold the neighbours' edge rows, as in the float32 driver.
+void mgpu_d8_flow_directions_flats_f64_band(const rdb200_comm *comm, double *d_band, uint8_t *d_dirs, int w, int hloc, double nodata,
+                                            int gt, int gb, bool alter, int *seam_iters) {
+  const char *what = "mgpu_d8_flow_directions_flats";
+  if (!d_dirs) fail("%s: null pointer", what);
+  check_band_args(what, comm, d_band, w, hloc, gt, gb);
+  Ctx &c = ctx();
+  gt = gt ? 1 : 0;
+  gb = gb ? 1 : 0;
+  const size_t n = (size_t)w * hloc;
+  DevBuf<float> k(n);
+  const float nd = mgpu_f64_keys_dev(comm, d_band, k.p, w, hloc, gt, gb, nodata, nullptr, nullptr);
+  d8_flow_directions_f64_dev(d_band, d_dirs, w, hloc, nodata);
+  DevBuf<int32_t> mask(alter ? n : 0);
+  const int iters = mgpu_dir_flats_band(comm, k.p, d_dirs, w, hloc, nd, gt, gb, alter, alter ? mask.p : nullptr);
+  k.reset();
+  if (alter) {
+    f64_float_steps_dev(d_band, mask.p, w, hloc);  // local rows 1 .. hloc-2: the owned rows, less the raster's edge rows
+    exchange_band_rows(comm, d_band, sizeof(double), w, hloc, gt, gb);
+    d8_flow_directions_f64_dev(d_band, d_dirs, w, hloc, nodata);
+  }
+  exchange_band_rows(comm, d_dirs, 1, w, hloc, gt, gb);
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  if (seam_iters) *seam_iters = iters;
+}
+
 // FlowAccumulation of a double band.  Methods 0 (D8) and 2 (D4) compare elevations only: the float32 band accumulation
 // on kappa_G.  The others compute with them: the double flow metric on a copy of the band whose ghost rows hold the
 // neighbours' edge rows, then the band accumulation of those proportions.  The caller's ghost rows are not read.

@@ -855,10 +855,15 @@ void d8_flow_directions_flats_dev(float *d_dem, uint8_t *d_dirs, int w, int h, f
   }
   DevBuf<int32_t> mask(n), labels(n);
   resolve_flats_dev(d_dem, w, h, nodata, mask.p, labels.p, false, d_dirs);
-  d8_flow_flats_kernel<<<c.num_sms * 16, 256, 0, c.stream>>>(mask.p, labels.p, d_dirs, w, h);
+  d8_flow_flats_dev(mask.p, labels.p, d_dirs, w, h);
+  RDB_CK(cudaStreamSynchronize(c.stream));
+}
+
+void d8_flow_flats_dev(const int32_t *d_mask, const int32_t *d_labels, uint8_t *d_dirs, int w, int h) {
+  Ctx &c = ctx();
+  d8_flow_flats_kernel<<<c.num_sms * 16, 256, 0, c.stream>>>(d_mask, d_labels, d_dirs, w, h);
   RDB_CK(cudaGetLastError());
   count_launch();
-  RDB_CK(cudaStreamSynchronize(c.stream));
 }
 
 }  // namespace rdb
@@ -1136,11 +1141,9 @@ void mgpu_resolve_flats_band(const rdb200_comm *comm, float *d_local, int w, int
 // barnes_flat_resolution_d8 (d8_flow_directions_flats_dev) over row bands.  The DEM's ghost rows hold the neighbours'
 // edge rows on entry.  Plain directions of the local raster first: its rows 0 / H-1 get the raster-edge rule, which is
 // right for the global top / bottom row and is replaced by the neighbours' directions in a ghost row.  The flats are
-// classified from the directions and resolved by the band protocol.  alter = 0: the increment mask crosses the seams
-// (d8_flow_flats compares a cell's mask with its same-label neighbours', ghost cells included; adjacent cells share a
-// local label exactly when they share a flat), then the NO_FLOW cells of the owned rows take their masked directions.
-// alter = 1: the increments go into the owned rows of the DEM, its edge rows cross the seams and the directions are
-// computed again.  On return the ghost rows of d_dirs (and, with alter = 1, of d_dem) hold the neighbours' edge rows.
+// resolved by mgpu_dir_flats_band.  alter = 1: the increments go into the owned rows of the DEM, its edge rows cross the
+// seams and the directions are computed again.  On return the ghost rows of d_dirs (and, with alter = 1, of d_dem) hold
+// the neighbours' edge rows.
 void mgpu_d8_flow_directions_flats_band(const rdb200_comm *comm, float *d_dem, uint8_t *d_dirs, int w, int hloc, float nodata,
                                         int gt, int gb, bool alter, int *seam_iters) {
   Ctx &c = ctx();
@@ -1149,29 +1152,40 @@ void mgpu_d8_flow_directions_flats_band(const rdb200_comm *comm, float *d_dem, u
   check_band_args(what, comm, d_dem, w, hloc, gt, gb);
   gt = gt ? 1 : 0;
   gb = gb ? 1 : 0;
-  auto exchange_rows = [&](void *p, size_t elem) { exchange_band_rows(comm, p, elem, w, hloc, gt, gb); };
   d8_flow_directions_dev(d_dem, d_dirs, w, hloc, nodata);
-  exchange_rows(d_dirs, 1);
+  const int iters = mgpu_dir_flats_band(comm, d_dem, d_dirs, w, hloc, nodata, gt, gb, alter, nullptr);
+  if (alter) {
+    exchange_band_rows(comm, d_dem, sizeof(float), w, hloc, gt, gb);
+    d8_flow_directions_dev(d_dem, d_dirs, w, hloc, nodata);
+  }
+  exchange_band_rows(comm, d_dirs, 1, w, hloc, gt, gb);
+  RDB_CK(cudaStreamSynchronize(c.stream));
+  if (seam_iters) *seam_iters = iters;
+}
+
+// The flats of a band's plain D8 directions d_dirs (owned rows computed; the ghost rows are exchanged here), classified
+// from the directions and resolved by the band protocol on the elevations d_dem, whose ghost rows hold the neighbours'
+// rows (float32 elevations, or the order keys of a float64 band).  alter = 0: the increment mask crosses the seams
+// (d8_flow_flats compares a cell's mask with its same-label neighbours', ghost cells included; adjacent cells share a
+// local label exactly when they share a flat), then the NO_FLOW cells take their masked directions.  alter = 1: the
+// increments go into d_dem as float ulps, or, with d_mask_out, the increment mask goes there and d_dem is not modified.
+// Returns the flag + height merge iterations.
+int mgpu_dir_flats_band(const rdb200_comm *comm, float *d_dem, uint8_t *d_dirs, int w, int hloc, float nodata, int gt, int gb,
+                        bool alter, int32_t *d_mask_out) {
+  Ctx &c = ctx();
+  exchange_band_rows(comm, d_dirs, 1, w, hloc, gt, gb);
   std::unique_ptr<rdb200_flats_state> s(flats_begin(d_dem, w, hloc, nodata, gt, gb, d_dirs));
   const int iters = flats_band_steps(comm, s.get(), true);
   if (alter) {
-    flats_apply(s.get());
-    s.reset();
-    exchange_rows(d_dem, sizeof(float));
-    d8_flow_directions_dev(d_dem, d_dirs, w, hloc, nodata);
+    flats_apply(s.get(), d_mask_out);
   } else {
     DevBuf<int32_t> mask((size_t)w * hloc);
     flats_apply(s.get(), mask.p);
-    exchange_rows(mask.p, sizeof(int32_t));
-    d8_flow_flats_kernel<<<c.num_sms * 16, 256, 0, c.stream>>>(mask.p, s->labels.p, d_dirs, w, hloc);
-    RDB_CK(cudaGetLastError());
-    count_launch();
+    exchange_band_rows(comm, mask.p, sizeof(int32_t), w, hloc, gt, gb);
+    d8_flow_flats_dev(mask.p, s->labels.p, d_dirs, w, hloc);
     RDB_CK(cudaStreamSynchronize(c.stream));
-    s.reset();
   }
-  exchange_rows(d_dirs, 1);
-  RDB_CK(cudaStreamSynchronize(c.stream));
-  if (seam_iters) *seam_iters = iters;
+  return iters;
 }
 
 }  // namespace rdb

@@ -1,7 +1,7 @@
 """float64 elevations on the GPU: ``FillDepressions``, ``PitMask``, ``HasDepressions``, ``ResolveFlats``,
-``FlowAccumulation`` (D8 / OCallaghanD8 / D4 / OCallaghanD4), ``FlowDirectionsD8``, ``FlowProportions`` and
-``TerrainAttribute`` for C-contiguous float64 ``rdarray``s, with the arguments, checks and messages of the float32
-functions in :mod:`richdem_b200`.
+``FlowAccumulation`` (D8 / OCallaghanD8 / D4 / OCallaghanD4), ``FlowDirectionsD8``, ``FlowDirectionsD8Resolved``,
+``FlatMask``, ``FlowProportions`` and ``TerrainAttribute`` for C-contiguous float64 ``rdarray``s, with the arguments,
+checks and messages of the float32 functions in :mod:`richdem_b200`.
 
 Each call gives what the reference's ``double`` templates give (the fill's zero sign aside, as for float32), within the
 float32 path's tolerances.  The stages that only compare elevations run the float engines on an order-preserving float
@@ -151,6 +151,31 @@ def FlowDirectionsD8(dem: rdarray) -> rdarray:
     _lib.check(_lib.lib().rdb200_d8_flow_directions_f64(_lib.ptr(d), _lib.ptr(out), w, h, _nodata_f64(dem)))
     out.no_data = 255
     return out
+
+
+def FlowDirectionsD8Resolved(dem: rdarray, alter: bool = False) -> rdarray:
+    """barnes_flat_resolution_d8<double, uint8_t>: D8 directions in which drainable flats flow along the Barnes (2014)
+    increment mask.  ``alter=True`` raises the flat cells of ``dem`` in place instead, as the reference does for a
+    double raster: m float-ulp steps (``nextafterf``) from the value rounded to float32, then the directions again."""
+    if type(dem) is not rdarray:
+        raise Exception("A richdem.rdarray or numpy.ndarray is required!")
+    d = _dem_f64(dem, "FlowDirectionsD8Resolved")
+    h, w = d.shape
+    out = rdarray(np.empty((h, w), np.uint8), meta_obj=dem, no_data=255)
+    _lib.check(_lib.lib().rdb200_d8_flow_directions_flats_f64(_lib.ptr(d), _lib.ptr(out), w, h, _nodata_f64(dem),
+                                                               int(bool(alter))))
+    out.no_data = 255
+    return out
+
+
+def FlatMask(dem: rdarray):
+    """GetFlatMask<double>: (mask, labels) int32 arrays; labels are equal within one flat, their values arbitrary."""
+    d = _dem_f64(dem, "FlatMask")
+    h, w = d.shape
+    mask = np.empty((h, w), np.int32)
+    labels = np.empty((h, w), np.int32)
+    _lib.check(_lib.lib().rdb200_get_flat_mask_f64(_lib.ptr(d), _lib.ptr(mask), _lib.ptr(labels), w, h, _nodata_f64(dem)))
+    return mask, labels
 
 
 def FlowProportions(dem: rdarray, method: Optional[str] = None, exponent: Optional[float] = None) -> rd3array:

@@ -841,8 +841,11 @@ def d8_flow_directions_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, n
     """FlowDirectionsD8Resolved over this rank's band.  ``local_dem`` is (g_top + owned + g_bot) x W and its ghost rows
     must hold the neighbours' elevation rows (:func:`fill_band` leaves them so).  ``alter=True`` raises the flat cells of
     the owned rows in place, as on one GPU.  Collective.  Returns (uint8 directions of the same local shape, whose ghost
-    rows hold the neighbours' edge-row directions, seam iterations)."""
+    rows hold the neighbours' edge-row directions, seam iterations).  A float64 band takes its directions from the doubles
+    and, with ``alter=True``, the reference's float steps (:func:`richdem_b200.f64.FlowDirectionsD8Resolved`)."""
     from . import _lib
+    if _is_f64(local_dem):
+        return _d8_flow_directions_band_f64(local_dem, g_top, g_bot, nodata, alter, group)
     assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
     _lib.use_torch_stream()
     h, w = local_dem.shape
@@ -999,6 +1002,17 @@ def _resolve_flats_band_f64(local_dem, g_top, g_bot, nodata, group):
     _lib.check(L.rdb200_mgpu_resolve_flats_epsilon_f64(cm.handle, local_dem.data_ptr(), w, h, float(nodata), int(g_top),
                                                        int(g_bot), C.byref(it)))
     return int(it.value)
+
+
+def _d8_flow_directions_band_f64(local_dem, g_top, g_bot, nodata, alter, group):
+    _lib, L = _f64_band(local_dem)
+    h, w = local_dem.shape
+    dirs = torch.empty((h, w), dtype=torch.uint8, device=local_dem.device)
+    it = C.c_int32(0)
+    cm = lib_comm(group, local_dem.is_cuda)
+    _lib.check(L.rdb200_mgpu_d8_flow_directions_flats_f64(cm.handle, local_dem.data_ptr(), dirs.data_ptr(), w, h, float(nodata),
+                                                          int(g_top), int(g_bot), int(bool(alter)), C.byref(it)))
+    return dirs, int(it.value)
 
 
 def _fa_band_f64(local_dem, g_top, g_bot, nodata, weights, group, return_stats, mid, xparam):
