@@ -14,7 +14,7 @@ from __future__ import annotations
 import copy
 import ctypes as C
 import datetime
-from typing import Any, Optional
+from typing import Any, Callable, NamedTuple, Optional, Tuple
 
 import numpy as np
 
@@ -99,94 +99,101 @@ class rd3array(_MetaArray):
         return obj
 
 
-# ---------------------------------------------------------------------------------------------
-def _dem_f32(dem: rdarray, what: str) -> np.ndarray:
+# ---- one body per stage; an element-type record carries what float32 and float64 DEMs differ in (f64.py binds _F64) -----
+class _Elem(NamedTuple):
+    dtype: type
+    suffix: str  # of the C symbols: rdb200_<stage>_<suffix>
+    nodata: Callable[[Any], float]  # a raster's no_data as the C ABI takes it
+    refusal: str  # the wrong-dtype message, with {what} and {dtype}
+    fa_valid: Tuple[str, ...]  # the methods FlowAccumulation lists as valid
+    fa_refused: Tuple[str, ...]  # known methods FlowAccumulation refuses for this element type
+    nodata_first: bool  # FlowAccumulation / FlowProportions read no_data before they check the method
+
+
+_F32 = _Elem(np.float32, "f32", lambda nd: float(np.float32(nd)),
+             "{what}: the H100 path is built for float32 elevations (got '{dtype}'); "
+             "convert with dem.astype('float32') -- there is no CPU fallback for other dtypes "
+             "(float64 rasters: richdem_b200.f64 computes the float64 answer).",
+             _DINF_METHODS + ("Quinn",) + _D8_METHODS + _D4_METHODS + _EXPONENT_METHODS + _OUT_OF_SCOPE_METHODS, (), False)
+_F64 = _Elem(np.float64, "f64", float,
+             "{what}: richdem_b200.f64 is built for float64 elevations (got '{dtype}'); "
+             "float32 rasters go through richdem_b200 itself.",
+             _D8_METHODS + _D4_METHODS, _DINF_METHODS + ("Quinn",) + _EXPONENT_METHODS + _OUT_OF_SCOPE_METHODS, True)
+
+
+def _dem(et: _Elem, dem: rdarray, what: str) -> np.ndarray:
     if dem.ndim != 2:
         raise RuntimeError("Array must have two dimensions!")  # pywrapper.hpp:118-119
-    if dem.dtype != np.float32:
-        raise Exception(
-            f"{what}: the H100 path is built for float32 elevations (got '{dem.dtype}'); "
-            "convert with dem.astype('float32') -- there is no CPU fallback for other dtypes "
-            "(float64 rasters: richdem_b200.f64 computes the float64 answer).")
+    if dem.dtype != et.dtype:
+        raise Exception(et.refusal.format(what=what, dtype=dem.dtype))
     if not dem.flags["C_CONTIGUOUS"]:
         raise Exception(f"{what}: the raster must be C-contiguous")
     return dem
 
 
-def _nodata_f32(dem) -> float:
+def _nodata(et: _Elem, dem) -> float:
     nd = dem.no_data
     if nd is None:
         print("Warning! no_data was None. Setting it to -9999!")  # reference :204-206
         nd = -9999
-    return float(np.float32(nd))
+    return et.nodata(nd)
 
 
-def FillDepressions(dem: rdarray, epsilon: bool = False, in_place: bool = False,
-                    topology: str = "D8") -> Optional[rdarray]:
-    """Fills all depressions in a DEM (reference FillDepressions, :381-422 -> PriorityFlood_Zhou2016 for ``D8``,
-    PriorityFlood_Barnes2014<D4> for ``D4``).  Returns the filled DEM unless ``in_place``."""
+def _check_topology(dem, topology: str) -> None:
     if type(dem) is not rdarray:
         raise Exception("A richdem.rdarray or numpy.ndarray is required!")
     if topology not in ["D8", "D4"]:
         raise Exception("Unknown topology!")
+
+
+def _fill_depressions(et, dem, epsilon, in_place, topology):
+    _check_topology(dem, topology)
     if epsilon:
         raise Exception("FillDepressions(epsilon=True) is outside the GPU hot path (SURVEY 8f-3)")
     if not in_place:
         dem = dem.copy()
     _add_analysis(dem, f"FillDepressions(dem, epsilon={epsilon})")
-    d = _dem_f32(dem, "FillDepressions")
+    d = _dem(et, dem, "FillDepressions")
     h, w = d.shape
-    fn = _lib.lib().rdb200_fill_depressions_d8_f32 if topology == "D8" else _lib.lib().rdb200_fill_depressions_d4_f32
+    fn = getattr(_lib.lib(), f"rdb200_fill_depressions_{topology.lower()}_{et.suffix}")
     _lib.check(fn(_lib.ptr(d), w, h))
     if not in_place:
         return dem
     return None
 
 
-def PitMask(dem: rdarray, topology: str = "D8") -> rdarray:
-    """richdem::pit_mask<topo> (depressions/Barnes2014.hpp:593-676; app rd_depressions_mask): uint8 mask of the cells
-    that lie in a depression, i.e. below the ``FillDepressions`` surface of ``dem`` (1), NoData cells (3) and all others
-    (0), with ``no_data`` 3 and the input's metadata.  ``dem`` is not modified."""
-    if type(dem) is not rdarray:
-        raise Exception("A richdem.rdarray or numpy.ndarray is required!")
-    if topology not in ["D8", "D4"]:
-        raise Exception("Unknown topology!")
-    d = _dem_f32(dem, "PitMask")
+def _pit_mask(et, dem, topology):
+    _check_topology(dem, topology)
+    d = _dem(et, dem, "PitMask")
     h, w = d.shape
     out = rdarray(np.empty((h, w), np.uint8), meta_obj=dem, no_data=3)
     _add_analysis(out, f"PitMask(dem, topology={topology})")
-    fn = _lib.lib().rdb200_pit_mask_d8_f32 if topology == "D8" else _lib.lib().rdb200_pit_mask_d4_f32
-    _lib.check(fn(_lib.ptr(d), _lib.ptr(out), w, h, _nodata_f32(dem)))
+    fn = getattr(_lib.lib(), f"rdb200_pit_mask_{topology.lower()}_{et.suffix}")
+    _lib.check(fn(_lib.ptr(d), _lib.ptr(out), w, h, _nodata(et, dem)))
     out.no_data = 3
     return out
 
 
-def HasDepressions(dem: rdarray, topology: str = "D8") -> bool:
-    """richdem::HasDepressions<topo> (depressions/Barnes2014.hpp:43-104; app rd_depressions_has): whether
-    ``FillDepressions`` would raise any cell.  NoData is not special, as in the reference."""
-    if type(dem) is not rdarray:
-        raise Exception("A richdem.rdarray or numpy.ndarray is required!")
-    if topology not in ["D8", "D4"]:
-        raise Exception("Unknown topology!")
-    d = _dem_f32(dem, "HasDepressions")
+def _has_depressions(et, dem, topology):
+    _check_topology(dem, topology)
+    d = _dem(et, dem, "HasDepressions")
     h, w = d.shape
     out = C.c_int32(0)
-    fn = _lib.lib().rdb200_has_depressions_d8_f32 if topology == "D8" else _lib.lib().rdb200_has_depressions_d4_f32
+    fn = getattr(_lib.lib(), f"rdb200_has_depressions_{topology.lower()}_{et.suffix}")
     _lib.check(fn(_lib.ptr(d), w, h, C.byref(out)))
     return bool(out.value)
 
 
-def ResolveFlats(dem: rdarray, in_place: bool = False) -> Optional[rdarray]:
-    """Imposes a local gradient on drainable flats (reference ResolveFlats, :461-487 ->
-    ResolveFlatsEpsilon)."""
+def _resolve_flats(et, dem, in_place):
     if type(dem) is not rdarray:
         raise Exception("A richdem.rdarray or numpy.ndarray is required!")
     if not in_place:
         dem = dem.copy()
     _add_analysis(dem, f"ResolveFlats(dem, in_place={in_place})")
-    d = _dem_f32(dem, "ResolveFlats")
+    d = _dem(et, dem, "ResolveFlats")
     h, w = d.shape
-    _lib.check(_lib.lib().rdb200_resolve_flats_epsilon_f32(_lib.ptr(d), w, h, _nodata_f32(dem)))
+    fn = getattr(_lib.lib(), f"rdb200_resolve_flats_epsilon_{et.suffix}")
+    _lib.check(fn(_lib.ptr(d), w, h, _nodata(et, dem)))
     if not in_place:
         return dem
     return None
@@ -210,44 +217,40 @@ def _accum_array(like, weights, in_place, shape):
     return accum, ones
 
 
-def FlowAccumulation(dem: rdarray, method: Optional[str] = None, exponent: Optional[float] = None,
-                     weights: Optional[rdarray] = None, in_place: bool = False) -> rdarray:
-    """Flow accumulation (reference FlowAccumulation, :490-596).  Methods on the H100 path:
-    ``D8`` / ``OCallaghanD8`` (FA_D8), ``Dinf`` / ``Tarboton`` (FA_Tarboton), ``D4`` / ``OCallaghanD4`` (FA_D4),
-    ``Quinn``, ``Holmgren`` (exponent), ``Freeman`` (exponent)."""
+def _flow_accumulation(et, dem, method, exponent, weights, in_place):
     if type(dem) is not rdarray:
         raise Exception("A richdem.rdarray or numpy.ndarray is required!")
     accum, ones = _accum_array(dem, weights, in_place, dem.shape)
     _add_analysis(accum, "FlowAccumulation(dem, method={0}, exponent={1}, weights={2}, in_place={3})".format(
         method, exponent, "None" if weights is None else "weights", in_place))
-    d = _dem_f32(dem, "FlowAccumulation")
+    d = _dem(et, dem, "FlowAccumulation")
     h, w = d.shape
     L = _lib.lib()
-    if method in _D8_METHODS:
-        _lib.check(L.rdb200_fa_d8_f32_f64(_lib.ptr(d), _lib.ptr(accum), w, h, _nodata_f32(dem), int(ones)))
-    elif method in _DINF_METHODS:
-        _lib.check(L.rdb200_fa_tarboton_f32_f64(_lib.ptr(d), _lib.ptr(accum), w, h, _nodata_f32(dem), int(ones)))
-    elif method in _D4_METHODS or method == "Quinn" or method in _EXPONENT_METHODS:
+    nd = _nodata(et, dem) if et.nodata_first else None
+    if method in et.fa_refused:
+        raise Exception(f'FlowAccumulation method "{method}" is not available for {et.dtype.__name__} rasters '
+                        "(it does arithmetic on elevation differences); valid methods here are: " + ", ".join(et.fa_valid))
+    if method in _OUT_OF_SCOPE_METHODS:
+        raise Exception(f'FlowAccumulation method "{method}" is outside the GPU hot path '
+                        "(random-walk metric; use the reference CPU implementation)")
+    if method not in et.fa_valid:
+        raise Exception("Invalid FlowAccumulation method. Valid methods are: " + ", ".join(et.fa_valid))
+    if not et.nodata_first:
+        nd = _nodata(et, dem)
+    if method in _D8_METHODS or method in _DINF_METHODS:
+        name = "d8" if method in _D8_METHODS else "tarboton"
+        _lib.check(getattr(L, f"rdb200_fa_{name}_{et.suffix}_f64")(_lib.ptr(d), _lib.ptr(accum), w, h, nd, int(ones)))
+    else:
         # FM_x into a device-resident proportions array + the generic accumulation (flow_accumulation.hpp:18-20,28)
         if ones:
             accum[...] = 1.0
-        nd = _nodata_f32(dem)
-        if method in _D4_METHODS:
-            _lib.check(L.rdb200_fa_d4_f32_f64(_lib.ptr(d), _lib.ptr(accum), w, h, nd))
-        elif method == "Quinn":
-            _lib.check(L.rdb200_fa_quinn_f32_f64(_lib.ptr(d), _lib.ptr(accum), w, h, nd))
-        else:
+        name = "d4" if method in _D4_METHODS else method.lower()
+        args = ()
+        if method in _EXPONENT_METHODS:
             if exponent is None:
                 raise Exception(f'FlowAccumulation method "{method}" requires an exponent!')
-            fn = L.rdb200_fa_freeman_f32_f64 if method == "Freeman" else L.rdb200_fa_holmgren_f32_f64
-            _lib.check(fn(_lib.ptr(d), _lib.ptr(accum), w, h, nd, float(exponent)))
-    elif method in _OUT_OF_SCOPE_METHODS:
-        raise Exception(f'FlowAccumulation method "{method}" is outside the GPU hot path '
-                        "(random-walk metric; use the reference CPU implementation)")
-    else:
-        raise Exception("Invalid FlowAccumulation method. Valid methods are: " +
-                        ", ".join(_DINF_METHODS + ("Quinn",) + _D8_METHODS + _D4_METHODS + _EXPONENT_METHODS +
-                                  _OUT_OF_SCOPE_METHODS))
+            args = (float(exponent),)
+        _lib.check(getattr(L, f"rdb200_fa_{name}_{et.suffix}_f64")(_lib.ptr(d), _lib.ptr(accum), w, h, nd, *args))
     accum.no_data = -1
     return accum
 
@@ -270,29 +273,24 @@ def FlowAccumFromProps(props: rd3array, weights: Optional[rdarray] = None, in_pl
     return accum
 
 
-def FlowProportions(dem: rdarray, method: Optional[str] = None, exponent: Optional[float] = None) -> rd3array:
-    """Flow proportions (reference FlowProportions, :650-732): (H, W, 9) float32, slot 0 holds
-    -2 NoData / -1 no flow / 0 has flow, slots 1..8 the share sent to D8 neighbour n."""
+def _flow_proportions(et, dem, method, exponent):
     if type(dem) is not rdarray:
         raise Exception("A richdem.rdarray or numpy.ndarray is required!")
     fprops = rd3array(np.empty(shape=dem.shape + (9,), dtype="float32"), meta_obj=dem, no_data=-2)
     _add_analysis(fprops, f"FlowProportions(dem, method={method}, exponent={exponent})")
-    d = _dem_f32(dem, "FlowProportions")
+    d = _dem(et, dem, "FlowProportions")
     h, w = d.shape
-    L = _lib.lib()
+    nd = _nodata(et, dem) if et.nodata_first else None
     if method in _D8_METHODS:
-        _lib.check(L.rdb200_fm_d8_f32(_lib.ptr(d), _lib.ptr(fprops), w, h, _nodata_f32(dem)))
+        name = "d8"
     elif method in _DINF_METHODS:
-        _lib.check(L.rdb200_fm_tarboton_f32(_lib.ptr(d), _lib.ptr(fprops), w, h, _nodata_f32(dem)))
+        name = "tarboton"
     elif method in _D4_METHODS:
-        _lib.check(L.rdb200_fm_d4_f32(_lib.ptr(d), _lib.ptr(fprops), w, h, _nodata_f32(dem)))
-    elif method == "Quinn":
-        _lib.check(L.rdb200_fm_quinn_f32(_lib.ptr(d), _lib.ptr(fprops), w, h, _nodata_f32(dem)))
-    elif method in _EXPONENT_METHODS:
-        if exponent is None:
+        name = "d4"
+    elif method == "Quinn" or method in _EXPONENT_METHODS:
+        if method != "Quinn" and exponent is None:
             raise Exception('FlowProportions method "' + method + '" requires an exponent!')
-        fn = L.rdb200_fm_freeman_f32 if method == "Freeman" else L.rdb200_fm_holmgren_f32
-        _lib.check(fn(_lib.ptr(d), _lib.ptr(fprops), w, h, _nodata_f32(dem), float(exponent)))
+        name = method.lower()
     elif method in _OUT_OF_SCOPE_METHODS:
         raise Exception(f'FlowProportions method "{method}" is outside the GPU hot path '
                         "(random-walk metric; use the reference CPU implementation)")
@@ -300,6 +298,10 @@ def FlowProportions(dem: rdarray, method: Optional[str] = None, exponent: Option
         raise Exception("Invalid FlowProportions method. Valid methods are: " +
                         ", ".join(_DINF_METHODS + ("Quinn",) + _D8_METHODS + _D4_METHODS + _EXPONENT_METHODS +
                                   _OUT_OF_SCOPE_METHODS))
+    if not et.nodata_first:
+        nd = _nodata(et, dem)
+    args = (float(exponent),) if method in _EXPONENT_METHODS else ()
+    _lib.check(getattr(_lib.lib(), f"rdb200_fm_{name}_{et.suffix}")(_lib.ptr(d), _lib.ptr(fprops), w, h, nd, *args))
     fprops.no_data = -2
     return fprops
 
@@ -315,15 +317,11 @@ def _terrain_attrib_id(attrib: str) -> int:
     return _TERRAIN_ATTRIBS[attrib]
 
 
-def TerrainAttribute(dem: rdarray, attrib: str, zscale: float = 1.0) -> rdarray:
-    """richdem.TerrainAttribute (wrappers/pyrichdem/richdem/__init__.py:735-794) over TA_* (methods/
-    terrain_attributes.hpp:370-538): Horn (1981) slope / aspect, Zevenbergen & Thorne (1987) curvatures; float32
-    result with no_data -9999.  Cell lengths come from the geotransform (1 x 1 when there is none, as in the
-    reference's wrap())."""
+def _terrain_attribute(et, dem, attrib, zscale):
     if type(dem) is not rdarray:
         raise Exception("A richdem.rdarray or numpy.ndarray is required!")
     attrib_id = _terrain_attrib_id(attrib)
-    d = _dem_f32(dem, "TerrainAttribute")
+    d = _dem(et, dem, "TerrainAttribute")
     h, w = d.shape
     gt = dem.geotransform
     if gt is None:
@@ -331,10 +329,98 @@ def TerrainAttribute(dem: rdarray, attrib: str, zscale: float = 1.0) -> rdarray:
         gt = [0, 1, 0, 0, 0, -1]
     result = rdarray(np.zeros((h, w), np.float32), meta_obj=dem, no_data=-9999)
     _add_analysis(result, f"TerrainAttribute(dem, attrib={attrib}, zscale={zscale})")
-    _lib.check(_lib.lib().rdb200_terrain_attribute_f32(attrib_id, _lib.ptr(d), _lib.ptr(result), w, h,
-                                                        _nodata_f32(dem), -9999.0, float(zscale), abs(float(gt[1])),
-                                                        abs(float(gt[5]))))
+    _lib.check(getattr(_lib.lib(), f"rdb200_terrain_attribute_{et.suffix}")(
+        attrib_id, _lib.ptr(d), _lib.ptr(result), w, h, _nodata(et, dem), -9999.0, float(zscale), abs(float(gt[1])),
+        abs(float(gt[5]))))
     return result
+
+
+def _flow_directions_d8(et, dem):
+    if type(dem) is not rdarray:
+        raise Exception("A richdem.rdarray or numpy.ndarray is required!")
+    d = _dem(et, dem, "FlowDirectionsD8")
+    h, w = d.shape
+    out = rdarray(np.empty((h, w), np.uint8), meta_obj=dem, no_data=255)
+    _lib.check(getattr(_lib.lib(), f"rdb200_d8_flow_directions_{et.suffix}")(_lib.ptr(d), _lib.ptr(out), w, h,
+                                                                            _nodata(et, dem)))
+    out.no_data = 255
+    return out
+
+
+def _flow_directions_d8_resolved(et, dem, alter):
+    if type(dem) is not rdarray:
+        raise Exception("A richdem.rdarray or numpy.ndarray is required!")
+    if et is _F32:  # the float32 function keeps its own refusal (no ndim check) and hands alter over as given
+        if dem.dtype != np.float32 or not dem.flags["C_CONTIGUOUS"]:
+            raise Exception("FlowDirectionsD8Resolved needs a C-contiguous float32 rdarray")
+        d, alter = dem, int(alter)
+    else:
+        d, alter = _dem(et, dem, "FlowDirectionsD8Resolved"), int(bool(alter))
+    h, w = d.shape
+    out = rdarray(np.empty((h, w), np.uint8), meta_obj=dem, no_data=255)
+    _lib.check(getattr(_lib.lib(), f"rdb200_d8_flow_directions_flats_{et.suffix}")(_lib.ptr(d), _lib.ptr(out), w, h,
+                                                                                  _nodata(et, dem), alter))
+    out.no_data = 255
+    return out
+
+
+def _flat_mask(et, dem):  # no rdarray check, in either module
+    d = _dem(et, dem, "FlatMask")
+    h, w = d.shape
+    mask = np.empty((h, w), np.int32)
+    labels = np.empty((h, w), np.int32)
+    _lib.check(getattr(_lib.lib(), f"rdb200_get_flat_mask_{et.suffix}")(_lib.ptr(d), _lib.ptr(mask), _lib.ptr(labels), w, h,
+                                                                       _nodata(et, dem)))
+    return mask, labels
+
+
+# ---------------------------------------------------------------------------------------------
+def FillDepressions(dem: rdarray, epsilon: bool = False, in_place: bool = False,
+                    topology: str = "D8") -> Optional[rdarray]:
+    """Fills all depressions in a DEM (reference FillDepressions, :381-422 -> PriorityFlood_Zhou2016 for ``D8``,
+    PriorityFlood_Barnes2014<D4> for ``D4``).  Returns the filled DEM unless ``in_place``."""
+    return _fill_depressions(_F32, dem, epsilon, in_place, topology)
+
+
+def PitMask(dem: rdarray, topology: str = "D8") -> rdarray:
+    """richdem::pit_mask<topo> (depressions/Barnes2014.hpp:593-676; app rd_depressions_mask): uint8 mask of the cells
+    that lie in a depression, i.e. below the ``FillDepressions`` surface of ``dem`` (1), NoData cells (3) and all others
+    (0), with ``no_data`` 3 and the input's metadata.  ``dem`` is not modified."""
+    return _pit_mask(_F32, dem, topology)
+
+
+def HasDepressions(dem: rdarray, topology: str = "D8") -> bool:
+    """richdem::HasDepressions<topo> (depressions/Barnes2014.hpp:43-104; app rd_depressions_has): whether
+    ``FillDepressions`` would raise any cell.  NoData is not special, as in the reference."""
+    return _has_depressions(_F32, dem, topology)
+
+
+def ResolveFlats(dem: rdarray, in_place: bool = False) -> Optional[rdarray]:
+    """Imposes a local gradient on drainable flats (reference ResolveFlats, :461-487 ->
+    ResolveFlatsEpsilon)."""
+    return _resolve_flats(_F32, dem, in_place)
+
+
+def FlowAccumulation(dem: rdarray, method: Optional[str] = None, exponent: Optional[float] = None,
+                     weights: Optional[rdarray] = None, in_place: bool = False) -> rdarray:
+    """Flow accumulation (reference FlowAccumulation, :490-596).  Methods on the H100 path:
+    ``D8`` / ``OCallaghanD8`` (FA_D8), ``Dinf`` / ``Tarboton`` (FA_Tarboton), ``D4`` / ``OCallaghanD4`` (FA_D4),
+    ``Quinn``, ``Holmgren`` (exponent), ``Freeman`` (exponent)."""
+    return _flow_accumulation(_F32, dem, method, exponent, weights, in_place)
+
+
+def FlowProportions(dem: rdarray, method: Optional[str] = None, exponent: Optional[float] = None) -> rd3array:
+    """Flow proportions (reference FlowProportions, :650-732): (H, W, 9) float32, slot 0 holds
+    -2 NoData / -1 no flow / 0 has flow, slots 1..8 the share sent to D8 neighbour n."""
+    return _flow_proportions(_F32, dem, method, exponent)
+
+
+def TerrainAttribute(dem: rdarray, attrib: str, zscale: float = 1.0) -> rdarray:
+    """richdem.TerrainAttribute (wrappers/pyrichdem/richdem/__init__.py:735-794) over TA_* (methods/
+    terrain_attributes.hpp:370-538): Horn (1981) slope / aspect, Zevenbergen & Thorne (1987) curvatures; float32
+    result with no_data -9999.  Cell lengths come from the geotransform (1 x 1 when there is none, as in the
+    reference's wrap())."""
+    return _terrain_attribute(_F32, dem, attrib, zscale)
 
 
 # ---- the reference's native cache format (host I/O; nothing runs on the GPU) ---------------------------------------------
@@ -390,29 +476,14 @@ def LoadNative(filename: str, dtype="float32") -> rdarray:
 # ---- C++-only functions of the path, exposed for completeness ---------------------------------
 def FlowDirectionsD8(dem: rdarray) -> rdarray:
     """richdem::d8_flow_directions (flowmet/d8_flowdirs.hpp:96-123): uint8 codes 0..8, 255 NoData."""
-    if type(dem) is not rdarray:
-        raise Exception("A richdem.rdarray or numpy.ndarray is required!")
-    d = _dem_f32(dem, "FlowDirectionsD8")
-    h, w = d.shape
-    out = rdarray(np.empty((h, w), np.uint8), meta_obj=dem, no_data=255)
-    _lib.check(_lib.lib().rdb200_d8_flow_directions_f32(_lib.ptr(d), _lib.ptr(out), w, h, _nodata_f32(dem)))
-    out.no_data = 255
-    return out
+    return _flow_directions_d8(_F32, dem)
 
 
 def FlowDirectionsD8Resolved(dem: rdarray, alter: bool = False) -> rdarray:
     """richdem::barnes_flat_resolution_d8 (flats/flat_resolution.hpp:588-607; the pipeline of apps/rd_d8_flowdirs.cpp):
     D8 directions in which drainable flats flow along the Barnes (2014) increment mask.  ``alter=True`` raises the
     flat cells of ``dem`` in place instead (d8_flats_alter_dem) and recomputes the directions."""
-    if type(dem) is not rdarray:
-        raise Exception("A richdem.rdarray or numpy.ndarray is required!")
-    if dem.dtype != np.float32 or not dem.flags["C_CONTIGUOUS"]:
-        raise Exception("FlowDirectionsD8Resolved needs a C-contiguous float32 rdarray")
-    h, w = dem.shape
-    out = rdarray(np.empty((h, w), np.uint8), meta_obj=dem, no_data=255)
-    _lib.check(_lib.lib().rdb200_d8_flow_directions_flats_f32(_lib.ptr(dem), _lib.ptr(out), w, h, _nodata_f32(dem), int(alter)))
-    out.no_data = 255
-    return out
+    return _flow_directions_d8_resolved(_F32, dem, alter)
 
 
 def D8FlowAccum(flowdirs: np.ndarray) -> rdarray:
@@ -428,10 +499,4 @@ def D8FlowAccum(flowdirs: np.ndarray) -> rdarray:
 
 def FlatMask(dem: rdarray):
     """richdem::GetFlatMask (flats/Barnes2014.hpp:398-467): (mask, labels) int32 arrays."""
-    d = _dem_f32(dem, "FlatMask")
-    h, w = d.shape
-    mask = np.empty((h, w), np.int32)
-    labels = np.empty((h, w), np.int32)
-    _lib.check(_lib.lib().rdb200_get_flat_mask_f32(_lib.ptr(d), _lib.ptr(mask), _lib.ptr(labels), w, h,
-                                                    _nodata_f32(dem)))
-    return mask, labels
+    return _flat_mask(_F32, dem)

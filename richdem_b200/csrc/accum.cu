@@ -1957,7 +1957,7 @@ static void fa_fused(const T *d_dem, double *d_accum, int w, int h, T nodata, bo
       return;
     }
   } else if (!dinf) {
-    fail("FA_D8 on doubles runs on float keys (fa_d8_f64_dev)");
+    fail("FA_D8 on doubles runs on float keys (fa_fused_dev)");
   }
   DevBuf<uint8_t> code(n);
   DevBuf<float> rmax;
@@ -2055,9 +2055,14 @@ static void fa_fused(const T *d_dem, double *d_accum, int w, int h, T nodata, bo
 void fa_fused_dev(const float *d_dem, double *d_accum, int w, int h, float nodata, bool ones, bool dinf) {
   fa_fused(d_dem, d_accum, w, h, nodata, ones, dinf);
 }
-// FA_Tarboton<double, double>: the same engine after a code pass on the doubles
-void fa_tarboton_f64_dev(const double *d_dem, double *d_accum, int w, int h, double nodata, bool ones) {
-  fa_fused(d_dem, d_accum, w, h, nodata, ones, true);
+// FA_Tarboton<double, double>: the same engine after a code pass on the doubles.  FA_D8<double, double> on the key raster:
+// the accumulation carries no elevation values.
+void fa_fused_dev(const double *d_dem, double *d_accum, int w, int h, double nodata, bool ones, bool dinf) {
+  if (dinf) return fa_fused(d_dem, d_accum, w, h, nodata, ones, true);
+  const size_t n = (size_t)w * h;
+  DevBuf<float> key(n);
+  const float nd = f64_keys_dev(d_dem, key.p, n, nodata, nullptr, nullptr);
+  fa_fused(key.p, d_accum, w, h, nd, ones, false);
 }
 
 // FlowAccumulation(props, accum) (reference methods/flow_accumulation_generic.hpp:33-100)
@@ -2339,9 +2344,7 @@ struct FaccState {
   // the owned rows are scattered here; the seam masks (set_ghost_codes) add the neighbours' shares to the edge rows.
   void begin_props(const float *d_dem, float nodata, double xparam, bool ones) {
     props.alloc(9 * n());
-    if (method == FA_BAND_D4) fm_d4_dev(d_dem, props.p, W, H, nodata);
-    else if (method == FA_BAND_HOLMGREN) fm_holmgren_dev(d_dem, props.p, W, H, nodata, xparam);
-    else fm_freeman_dev(d_dem, props.p, W, H, nodata, xparam);
+    fm_method_dev(method, d_dem, props.p, W, H, nodata, xparam);
     init_props_walk(props.p, ones);
   }
 

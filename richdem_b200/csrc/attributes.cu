@@ -184,8 +184,8 @@ void terrain_attribute_dev(int attribute_id, const float *d_dem, float *d_out, i
                            float zscale, double cell_x, double cell_y) {
   terrain_attribute_any(attribute_id, d_dem, d_out, w, h, nodata_in, nodata_out, zscale, cell_x, cell_y);
 }
-void terrain_attribute_f64_dev(int attribute_id, const double *d_dem, float *d_out, int w, int h, double nodata_in,
-                               float nodata_out, float zscale, double cell_x, double cell_y) {
+void terrain_attribute_dev(int attribute_id, const double *d_dem, float *d_out, int w, int h, double nodata_in,
+                           float nodata_out, float zscale, double cell_x, double cell_y) {
   terrain_attribute_any(attribute_id, d_dem, d_out, w, h, nodata_in, nodata_out, zscale, cell_x, cell_y);
 }
 

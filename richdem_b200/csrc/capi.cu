@@ -4,6 +4,7 @@
 
 #include <algorithm>
 #include <cstdlib>
+#include <type_traits>
 
 namespace rdb {
 
@@ -234,19 +235,27 @@ static int raster_call(Side side, const char *null_msg, std::initializer_list<co
   return raster_call(side, null_msg, ptrs, w, h, [] {}, body);
 }
 
-// ---- the stages, each for host and device arrays ------------------------------------------------------------------
+// ---- the stages, each for host and device arrays and T = float or double elevations -------------------------------
+// A float64 stage runs the float engines on order-preserving float keys (f64.cu) where it only compares elevations, and
+// the kernels' double instantiations where it does arithmetic on them (DESIGN §0.1, §0.2).
 
-static int fill_depressions(Side side, float *dem, int32_t w, int32_t h, bool topo4) {
+// reference depressions/depressions.hpp:13-21 -> Zhou2016.hpp:125-191 (D8) / Barnes2014.hpp:230-304 (D4)
+template <class T>
+static int fill_depressions(Side side, T *dem, int32_t w, int32_t h, bool topo4) {
   return raster_call(side, "fill_depressions: null dem", {dem}, w, h,
                      [&](Arrays &a, size_t n) { fill_depressions_dev(a.inout(dem, n), w, h, topo4); });
 }
 
-static int pit_mask(Side side, const float *dem, uint8_t *mask, int32_t w, int32_t h, float nodata, bool topo4) {
+// reference depressions/Barnes2014.hpp:593-676 (pit_mask<topo>)
+template <class T>
+static int pit_mask(Side side, const T *dem, uint8_t *mask, int32_t w, int32_t h, T nodata, bool topo4) {
   return raster_call(side, "pit_mask: null pointer", {dem, mask}, w, h,
                      [&](Arrays &a, size_t n) { pit_mask_dev(a.in(dem, n), a.out(mask, n), w, h, nodata, topo4); });
 }
 
-static int has_depressions(Side side, const float *dem, int32_t w, int32_t h, int32_t *out, bool topo4) {
+// reference depressions/Barnes2014.hpp:43-104 (HasDepressions<topo>)
+template <class T>
+static int has_depressions(Side side, const T *dem, int32_t w, int32_t h, int32_t *out, bool topo4) {
   bool any = false;
   const int rc = raster_call(side, "has_depressions: null pointer", {dem, out}, w, h,
                              [&](Arrays &a, size_t n) { any = has_depressions_dev(a.in(dem, n), w, h, topo4); });
@@ -254,18 +263,31 @@ static int has_depressions(Side side, const float *dem, int32_t w, int32_t h, in
   return rc;
 }
 
-static int resolve_flats_epsilon(Side side, float *dem, int32_t w, int32_t h, float nodata) {
-  return raster_call(side, "resolve_flats: null dem", {dem}, w, h, [&](Arrays &a, size_t n) {
-    resolve_flats_dev(a.inout(dem, n), w, h, nodata, nullptr, nullptr, true);
+// reference flats/flats.hpp:21-28 -> flats/Barnes2014.hpp:398-467 (GetFlatMask) + :496-550 (apply)
+template <class T>
+static int resolve_flats_epsilon(Side side, T *dem, int32_t w, int32_t h, T nodata) {
+  return raster_call(side, "resolve_flats: null dem", {dem}, w, h,
+                     [&](Arrays &a, size_t n) { resolve_flats_epsilon_dev(a.inout(dem, n), w, h, nodata); });
+}
+
+// reference flats/Barnes2014.hpp:398-467 (GetFlatMask)
+template <class T>
+static int get_flat_mask(Side side, const T *dem, int32_t *flat_mask, int32_t *labels, int32_t w, int32_t h, T nodata) {
+  return raster_call(side, "get_flat_mask: null pointer", {dem, flat_mask, labels}, w, h, [&](Arrays &a, size_t n) {
+    get_flat_mask_dev(a.in(dem, n), a.out(flat_mask, n), a.out(labels, n), w, h, nodata);
   });
 }
 
-static int d8_flow_directions(Side side, const float *dem, uint8_t *dirs, int32_t w, int32_t h, float nodata) {
+// reference flowmet/d8_flowdirs.hpp:32-123 (d8_flow_directions)
+template <class T>
+static int d8_flow_directions(Side side, const T *dem, uint8_t *dirs, int32_t w, int32_t h, T nodata) {
   return raster_call(side, "d8_flow_directions: null pointer", {dem, dirs}, w, h,
                      [&](Arrays &a, size_t n) { d8_flow_directions_dev(a.in(dem, n), a.out(dirs, n), w, h, nodata); });
 }
 
-static int d8_flow_directions_flats(Side side, float *dem, uint8_t *dirs, int32_t w, int32_t h, float nodata, int32_t alter) {
+// reference flats/flat_resolution.hpp:588-607 (barnes_flat_resolution_d8); dem is written only with alter
+template <class T>
+static int d8_flow_directions_flats(Side side, T *dem, uint8_t *dirs, int32_t w, int32_t h, T nodata, int32_t alter) {
   return raster_call(side, "d8_flow_directions_flats: null pointer", {dem, dirs}, w, h, [&](Arrays &a, size_t n) {
     d8_flow_directions_flats_dev(alter ? a.inout(dem, n) : a.in(dem, n), a.out(dirs, n), w, h, nodata, alter != 0);
   });
@@ -277,25 +299,16 @@ static int d8_flow_accum(Side side, const uint8_t *dirs, int32_t *area, int32_t 
 }
 
 // method: 0 FM_D8, 1 FM_Tarboton, 2 FM_D4, 3 FM_Holmgren (FM_Quinn = exponent 1), 4 FM_Freeman
-static void fm_dispatch_dev(int method, const float *d_dem, float *d_props, int w, int h, float nodata, double xparam) {
-  switch (method) {
-    case 0: fm_d8_dev(d_dem, d_props, w, h, nodata); break;
-    case 1: fm_tarboton_dev(d_dem, d_props, w, h, nodata); break;
-    case 2: fm_d4_dev(d_dem, d_props, w, h, nodata); break;
-    case 3: fm_holmgren_dev(d_dem, d_props, w, h, nodata, xparam); break;
-    case 4: fm_freeman_dev(d_dem, d_props, w, h, nodata, xparam); break;
-    default: fail("unknown flow metric %d", method);
-  }
-}
-
-static int fm(Side side, int method, const float *dem, float *props, int32_t w, int32_t h, float nodata, double xparam = 0) {
+template <class T>
+static int fm(Side side, int method, const T *dem, float *props, int32_t w, int32_t h, T nodata, double xparam = 0) {
   return raster_call(side, "flow metric: null pointer", {dem, props}, w, h, [&](Arrays &a, size_t n) {
-    fm_dispatch_dev(method, a.in(dem, n), a.out(props, 9 * n), w, h, nodata, xparam);
+    fm_method_dev(method, a.in(dem, n), a.out(props, 9 * n), w, h, nodata, xparam);
   });
 }
 
-// TA_* (reference methods/terrain_attributes.hpp:370-538): one stencil pass, 4 B in + 4 B out per cell
-static int terrain_attribute(Side side, int32_t attribute, const float *dem, float *out, int32_t w, int32_t h, float nodata_in,
+// TA_* (reference methods/terrain_attributes.hpp:370-538): one stencil pass, sizeof(T) B in + 4 B out per cell
+template <class T>
+static int terrain_attribute(Side side, int32_t attribute, const T *dem, float *out, int32_t w, int32_t h, T nodata_in,
                              float nodata_out, float zscale, double cell_x, double cell_y) {
   return raster_call(side, "terrain attribute: null pointer", {dem, out}, w, h, [&](Arrays &a, size_t n) {
     terrain_attribute_dev(attribute, a.in(dem, n), a.out(out, n), w, h, nodata_in, nodata_out, zscale, cell_x, cell_y);
@@ -303,14 +316,25 @@ static int terrain_attribute(Side side, int32_t attribute, const float *dem, flo
 }
 
 // FA_<metric> = FM_<metric> into a device-side proportions array + the generic accumulation
-// (reference methods/flow_accumulation.hpp:18-20,28: `Array3D<float> props(elevations); FM_x(...); FlowAccumulation(...)`)
-static void fa_via_props_dev(int method, const float *d_dem, double *d_accum, int w, int h, float nodata, double xparam) {
+// (reference methods/flow_accumulation.hpp:18-20,28: `Array3D<float> props(elevations); FM_x(...); FlowAccumulation(...)`).
+// On doubles, D8 and D4 compare elevations only and take the key route: FA_D8 by the fused engine, FA_D4 by the float
+// FM_D4 of the keys (accum holds the weights).
+template <class T>
+static void fa_via_props_dev(int method, const T *d_dem, double *d_accum, int w, int h, T nodata, double xparam) {
+  if constexpr (std::is_same_v<T, double>) {
+    if (method == 0) return fa_fused_dev(d_dem, d_accum, w, h, nodata, false, false);
+    if (method == 2) {
+      DevBuf<float> key((size_t)w * h);
+      const float nd = f64_keys_dev(d_dem, key.p, (size_t)w * h, nodata, nullptr, nullptr);
+      return fa_via_props_dev(2, key.p, d_accum, w, h, nd, 0.0);
+    }
+  }
   DevBuf<float> p(9 * (size_t)w * h);
-  fm_dispatch_dev(method, d_dem, p.p, w, h, nodata, xparam);
+  fm_method_dev(method, d_dem, p.p, w, h, nodata, xparam);
   flow_accumulation_props_dev(p.p, d_accum, w, h);
 }
-static int fa_via_props(Side side, int method, const float *dem, double *accum, int32_t w, int32_t h, float nodata,
-                        double xparam) {
+template <class T>
+static int fa_via_props(Side side, int method, const T *dem, double *accum, int32_t w, int32_t h, T nodata, double xparam) {
   return raster_call(side, "flow accumulation: null pointer", {dem, accum}, w, h, [&](Arrays &a, size_t n) {
     fa_via_props_dev(method, a.in(dem, n), a.inout(accum, n), w, h, nodata, xparam);
   });
@@ -323,123 +347,10 @@ static int flow_accumulation_props(Side side, const float *props, double *accum,
 }
 
 // FA_D8 / FA_Tarboton by the fused engines; with ones the accumulator is not read, only written
-static int fa_fused(Side side, const float *dem, double *accum, int32_t w, int32_t h, float nodata, int32_t ones, bool dinf) {
+template <class T>
+static int fa_fused(Side side, const T *dem, double *accum, int32_t w, int32_t h, T nodata, int32_t ones, bool dinf) {
   return raster_call(side, "flow accumulation: null pointer", {dem, accum}, w, h, [&](Arrays &a, size_t n) {
     fa_fused_dev(a.in(dem, n), ones ? a.out(accum, n) : a.inout(accum, n), w, h, nodata, ones != 0, dinf);
-  });
-}
-
-// ---- float64 rasters (f64.cu): the float engines on kappa(Z), kappa an order-preserving map to float keys ------------
-
-// reference depressions/depressions.hpp:13-21 -> Zhou2016.hpp:125-191 (D8) / Barnes2014.hpp:230-304 (D4), T = double
-static int fill_depressions_f64(Side side, double *dem, int32_t w, int32_t h, bool topo4) {
-  return raster_call(side, "fill_depressions: null dem", {dem}, w, h,
-                     [&](Arrays &a, size_t n) { fill_depressions_f64_dev(a.inout(dem, n), w, h, topo4); });
-}
-
-// reference depressions/Barnes2014.hpp:593-676 (pit_mask<topo>, T = double)
-static int pit_mask_f64(Side side, const double *dem, uint8_t *mask, int32_t w, int32_t h, double nodata, bool topo4) {
-  return raster_call(side, "pit_mask: null pointer", {dem, mask}, w, h,
-                     [&](Arrays &a, size_t n) { pit_mask_f64_dev(a.in(dem, n), a.out(mask, n), w, h, nodata, topo4); });
-}
-
-// reference depressions/Barnes2014.hpp:43-104 (HasDepressions<topo>, T = double)
-static int has_depressions_f64(Side side, const double *dem, int32_t w, int32_t h, int32_t *out, bool topo4) {
-  bool any = false;
-  const int rc = raster_call(side, "has_depressions: null pointer", {dem, out}, w, h,
-                             [&](Arrays &a, size_t n) { any = has_depressions_f64_dev(a.in(dem, n), w, h, topo4); });
-  if (rc == 0) *out = any ? 1 : 0;
-  return rc;
-}
-
-// reference flats/flats.hpp:21-28 -> flats/Barnes2014.hpp:398-467 (GetFlatMask) + :496-550 (apply), T = double
-static int resolve_flats_epsilon_f64(Side side, double *dem, int32_t w, int32_t h, double nodata) {
-  return raster_call(side, "resolve_flats: null dem", {dem}, w, h,
-                     [&](Arrays &a, size_t n) { resolve_flats_f64_dev(a.inout(dem, n), w, h, nodata); });
-}
-
-// reference flowmet/d8_flowdirs.hpp:32-123 (d8_flow_directions<double, uint8_t>)
-static int d8_flow_directions_f64(Side side, const double *dem, uint8_t *dirs, int32_t w, int32_t h, double nodata) {
-  return raster_call(side, "d8_flow_directions: null pointer", {dem, dirs}, w, h,
-                     [&](Arrays &a, size_t n) { d8_flow_directions_f64_dev(a.in(dem, n), a.out(dirs, n), w, h, nodata); });
-}
-
-// reference flats/Barnes2014.hpp:398-467 (GetFlatMask, T = double)
-static int get_flat_mask_f64(Side side, const double *dem, int32_t *flat_mask, int32_t *labels, int32_t w, int32_t h,
-                             double nodata) {
-  return raster_call(side, "get_flat_mask: null pointer", {dem, flat_mask, labels}, w, h, [&](Arrays &a, size_t n) {
-    get_flat_mask_f64_dev(a.in(dem, n), a.out(flat_mask, n), a.out(labels, n), w, h, nodata);
-  });
-}
-
-// reference flats/flat_resolution.hpp:588-607 (barnes_flat_resolution_d8<double, uint8_t>); dem is written only with alter
-static int d8_flow_directions_flats_f64(Side side, double *dem, uint8_t *dirs, int32_t w, int32_t h, double nodata, int32_t alter) {
-  return raster_call(side, "d8_flow_directions_flats: null pointer", {dem, dirs}, w, h, [&](Arrays &a, size_t n) {
-    d8_flow_directions_flats_f64_dev(alter ? a.inout(dem, n) : a.in(dem, n), a.out(dirs, n), w, h, nodata, alter != 0);
-  });
-}
-
-// reference methods/flow_accumulation.hpp:27 (FA_D8<double, double>: OCallaghan1984.hpp:13-91 + flow_accumulation_generic.hpp:33-100)
-static int fa_d8_f64(Side side, const double *dem, double *accum, int32_t w, int32_t h, double nodata, int32_t ones) {
-  return raster_call(side, "flow accumulation: null pointer", {dem, accum}, w, h, [&](Arrays &a, size_t n) {
-    fa_d8_f64_dev(a.in(dem, n), ones ? a.out(accum, n) : a.inout(accum, n), w, h, nodata, ones != 0);
-  });
-}
-
-// reference methods/flow_accumulation.hpp:28 (FA_D4<double, double>: OCallaghan1984.hpp:89-91 + the generic accumulation)
-static void fa_d4_f64_dev(const double *d_dem, double *d_accum, int w, int h, double nodata) {
-  DevBuf<float> key((size_t)w * h);
-  const float nd = f64_keys_dev(d_dem, key.p, (size_t)w * h, nodata, nullptr, nullptr);
-  fa_via_props_dev(2, key.p, d_accum, w, h, nd, 0);
-}
-static int fa_d4_f64(Side side, const double *dem, double *accum, int32_t w, int32_t h, double nodata) {
-  return raster_call(side, "flow accumulation: null pointer", {dem, accum}, w, h,
-                     [&](Arrays &a, size_t n) { fa_d4_f64_dev(a.in(dem, n), a.inout(accum, n), w, h, nodata); });
-}
-
-// ---- float64 D-infinity, MFD and terrain attributes: the float kernels' double instantiations (no keys: these stages do
-// arithmetic on the elevations, DESIGN §0.2).  Argument order and checks as the float stages above.
-
-// reference flowmet/*.hpp with E = double; method numbered as fm_dispatch_dev
-static int fm_f64(Side side, int method, const double *dem, float *props, int32_t w, int32_t h, double nodata, double xparam = 0) {
-  return raster_call(side, "flow metric: null pointer", {dem, props}, w, h, [&](Arrays &a, size_t n) {
-    fm_method_f64_dev(method, a.in(dem, n), a.out(props, 9 * n), w, h, nodata, xparam);
-  });
-}
-
-// methods/flow_accumulation.hpp:16-20 with E = double: FM_x on the doubles into device-side proportions + the generic
-// accumulation; methods 0 and 2 take the key route of FA_D8 / FA_D4 (accum holds the weights)
-static void fa_method_f64_dev(int method, const double *d_dem, double *d_accum, int w, int h, double nodata, double xparam) {
-  if (method == 0) {
-    fa_d8_f64_dev(d_dem, d_accum, w, h, nodata, false);
-  } else if (method == 2) {
-    fa_d4_f64_dev(d_dem, d_accum, w, h, nodata);
-  } else {
-    DevBuf<float> p(9 * (size_t)w * h);
-    fm_method_f64_dev(method, d_dem, p.p, w, h, nodata, xparam);
-    flow_accumulation_props_dev(p.p, d_accum, w, h);
-  }
-}
-static int fa_method_f64(Side side, int method, const double *dem, double *accum, int32_t w, int32_t h, double nodata,
-                         double xparam) {
-  return raster_call(side, "flow accumulation: null pointer", {dem, accum}, w, h, [&](Arrays &a, size_t n) {
-    fa_method_f64_dev(method, a.in(dem, n), a.inout(accum, n), w, h, nodata, xparam);
-  });
-}
-
-// methods/flow_accumulation.hpp:16 (FA_Tarboton<double, double>): the fused D-infinity engine after a code pass on the
-// doubles; ones as fa_fused
-static int fa_tarboton_f64(Side side, const double *dem, double *accum, int32_t w, int32_t h, double nodata, int32_t ones) {
-  return raster_call(side, "flow accumulation: null pointer", {dem, accum}, w, h, [&](Arrays &a, size_t n) {
-    fa_tarboton_f64_dev(a.in(dem, n), ones ? a.out(accum, n) : a.inout(accum, n), w, h, nodata, ones != 0);
-  });
-}
-
-// methods/terrain_attributes.hpp:370-538 with T = double: 8 B in + 4 B out per cell
-static int terrain_attribute_f64(Side side, int32_t attribute, const double *dem, float *out, int32_t w, int32_t h,
-                                 double nodata_in, float nodata_out, float zscale, double cell_x, double cell_y) {
-  return raster_call(side, "terrain attribute: null pointer", {dem, out}, w, h, [&](Arrays &a, size_t n) {
-    terrain_attribute_f64_dev(attribute, a.in(dem, n), a.out(out, n), w, h, nodata_in, nodata_out, zscale, cell_x, cell_y);
   });
 }
 
@@ -456,9 +367,11 @@ static int f64_order_keys(Side side, const double *dem, float *keys, int32_t w, 
   return rc;
 }
 
-// ---- row bands: the drivers take device pointers and check the band geometry themselves ----------------------------
+// ---- row bands: the drivers take device pointers and check the band geometry themselves; the float64 drivers check
+// every argument before kappa_G's first collective ------------------------------------------------------------------
 
-static int mgpu_fill(const rdb200_comm *comm, float *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb, int32_t row0,
+template <class T>
+static int mgpu_fill(const rdb200_comm *comm, T *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb, int32_t row0,
                      int32_t height, int32_t *exchange_rounds, bool topo4) {
   int xr = 0;
   const int rc = raster_call(Side::device, "mgpu_fill: null pointer", {d_band}, w, rows, [&](Arrays &, size_t) {
@@ -468,14 +381,16 @@ static int mgpu_fill(const rdb200_comm *comm, float *d_band, int32_t w, int32_t 
   return rc;
 }
 
-static int mgpu_pit_mask(const rdb200_comm *comm, const float *d_band, uint8_t *d_band_mask, int32_t w, int32_t rows, float nodata,
+template <class T>
+static int mgpu_pit_mask(const rdb200_comm *comm, const T *d_band, uint8_t *d_band_mask, int32_t w, int32_t rows, T nodata,
                          int32_t gt, int32_t gb, int32_t row0, int32_t height, bool topo4) {
   return raster_call(Side::device, "mgpu_pit_mask: null pointer", {comm, d_band, d_band_mask}, w, rows, [&](Arrays &, size_t) {
     mgpu_pit_mask_band(comm, d_band, d_band_mask, w, rows, nodata, gt, gb, row0, height, topo4);
   });
 }
 
-static int mgpu_has_depressions(const rdb200_comm *comm, const float *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb,
+template <class T>
+static int mgpu_has_depressions(const rdb200_comm *comm, const T *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb,
                                 int32_t row0, int32_t height, int32_t *out, bool topo4) {
   bool any = false;
   const int rc = raster_call(Side::device, "mgpu_has_depressions: null pointer", {comm, d_band, out}, w, rows,
@@ -486,32 +401,82 @@ static int mgpu_has_depressions(const rdb200_comm *comm, const float *d_band, in
   return rc;
 }
 
-// float64 bands: every argument is checked before kappa_G's first collective
-static int mgpu_fill_f64(const rdb200_comm *comm, double *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb, int32_t row0,
-                         int32_t height, int32_t *exchange_rounds, bool topo4) {
-  int xr = 0;
-  const int rc = raster_call(Side::device, "mgpu_fill: null pointer", {d_band}, w, rows, [&](Arrays &, size_t) {
-    mgpu_fill_f64_band(comm, d_band, w, rows, gt, gb, row0, height, &xr, topo4);
-  });
-  if (rc == 0 && exchange_rounds) *exchange_rounds = xr;
+template <class T>
+static int mgpu_resolve_flats_epsilon(const rdb200_comm *comm, T *d_band, int32_t w, int32_t rows, T nodata, int32_t gt,
+                                      int32_t gb, int32_t *seam_iterations) {
+  int it = 0;
+  const int rc = raster_call(Side::device, "mgpu_resolve_flats: null pointer", {comm, d_band}, w, rows,
+                             [&](Arrays &, size_t) { mgpu_resolve_flats_band(comm, d_band, w, rows, nodata, gt, gb, &it); });
+  if (rc == 0 && seam_iterations) *seam_iterations = it;
   return rc;
 }
 
-static int mgpu_pit_mask_f64(const rdb200_comm *comm, const double *d_band, uint8_t *d_band_mask, int32_t w, int32_t rows,
-                             double nodata, int32_t gt, int32_t gb, int32_t row0, int32_t height, bool topo4) {
-  return raster_call(Side::device, "mgpu_pit_mask: null pointer", {comm, d_band, d_band_mask}, w, rows, [&](Arrays &, size_t) {
-    mgpu_pit_mask_f64_band(comm, d_band, d_band_mask, w, rows, nodata, gt, gb, row0, height, topo4);
-  });
+template <class T>
+static int mgpu_d8_flow_directions_flats(const rdb200_comm *comm, T *d_band_dem, uint8_t *d_band_dirs, int32_t w, int32_t rows,
+                                         T nodata, int32_t gt, int32_t gb, int32_t alter, int32_t *seam_iterations) {
+  int it = 0;
+  const int rc = raster_call(Side::device, "mgpu_d8_flow_directions_flats: null pointer", {comm, d_band_dem, d_band_dirs}, w, rows,
+                             [&](Arrays &, size_t) {
+                               mgpu_d8_flow_directions_flats_band(comm, d_band_dem, d_band_dirs, w, rows, nodata, gt, gb,
+                                                                  alter != 0, &it);
+                             });
+  if (rc == 0 && seam_iterations) *seam_iterations = it;
+  return rc;
 }
 
-static int mgpu_has_depressions_f64(const rdb200_comm *comm, const double *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb,
-                                    int32_t row0, int32_t height, int32_t *out, bool topo4) {
-  bool any = false;
-  const int rc = raster_call(Side::device, "mgpu_has_depressions: null pointer", {comm, d_band, out}, w, rows,
-                             [&](Arrays &, size_t) {
-                               any = mgpu_has_depressions_f64_band(comm, d_band, w, rows, gt, gb, row0, height, topo4);
-                             });
-  if (rc == 0) *out = any ? 1 : 0;
+// FM_x and TA_x over row bands: one exchange of the DEM's edge rows gives every owned cell its whole 3 x 3 neighbourhood,
+// and a local edge row is a raster edge row exactly when it is not a ghost row, so the single-GPU kernel on the local raster
+// gives the owned rows the single-GPU bits.
+template <class T>
+static int mgpu_fm_method(const rdb200_comm *comm, int32_t method, T *d_band_dem, float *d_band_props9, int32_t w, int32_t rows,
+                          T nodata, int32_t gt, int32_t gb, double xparam) {
+  return raster_call(
+      Side::device, "mgpu_fm_method: null pointer", {d_band_props9, comm, d_band_dem}, w, rows,
+      [&] {
+        check_band_args("mgpu_fm_method", comm, d_band_dem, w, rows, gt, gb);
+        if (method < 0 || method > 4) fail("unknown flow metric %d", method);
+      },
+      [&](Arrays &, size_t) {
+        exchange_band_rows(comm, d_band_dem, sizeof(T), w, rows, gt, gb);
+        fm_method_dev(method, d_band_dem, d_band_props9, w, rows, nodata, xparam);
+      });
+}
+
+template <class T>
+static int mgpu_terrain_attribute(const rdb200_comm *comm, int32_t attribute, T *d_band_dem, float *d_band_out, int32_t w,
+                                  int32_t rows, T nodata_in, float nodata_out, float zscale, double cell_x, double cell_y,
+                                  int32_t gt, int32_t gb) {
+  return raster_call(
+      Side::device, "mgpu_terrain_attribute: null pointer", {d_band_out, comm, d_band_dem}, w, rows,
+      [&] {
+        check_band_args("mgpu_terrain_attribute", comm, d_band_dem, w, rows, gt, gb);
+        if (attribute < RDB200_TA_SLOPE_RISERUN || attribute > RDB200_TA_PROFILE_CURVATURE)
+          fail("unknown terrain attribute %d", attribute);
+        if (!(cell_x > 0) || !(cell_y > 0))
+          fail("terrain attribute: cell lengths must be positive (got %g x %g)", cell_x, cell_y);
+      },
+      [&](Arrays &, size_t) {
+        exchange_band_rows(comm, d_band_dem, sizeof(T), w, rows, gt, gb);
+        terrain_attribute_dev(attribute, d_band_dem, d_band_out, w, rows, nodata_in, nodata_out, zscale, cell_x, cell_y);
+      });
+}
+
+// The float32 driver checks the method as it begins; the float64 driver needs the communicator, the band and the method
+// checked before kappa_G's first collective.
+template <class T>
+static int mgpu_fa_method(const rdb200_comm *comm, const T *d_dem, double *d_accum, int32_t w, int32_t rows, T nodata, int32_t gt,
+                          int32_t gb, int32_t method, double xparam, int32_t ones, int32_t *exchange_rounds) {
+  constexpr bool keyed = std::is_same_v<T, double>;
+  int xr = 0;
+  const int rc = raster_call(
+      Side::device, "mgpu_fa: null pointer", {keyed ? (const void *)comm : d_dem, d_dem, d_accum}, w, rows,
+      [&] {
+        if (!keyed) return;
+        check_band_args("mgpu_fa", comm, d_dem, w, rows, gt, gb);
+        check_fa_method(method, xparam);
+      },
+      [&](Arrays &, size_t) { mgpu_fa_band(comm, d_dem, d_accum, w, rows, nodata, gt, gb, method, xparam, ones != 0, &xr); });
+  if (rc == 0 && exchange_rounds) *exchange_rounds = xr;
   return rc;
 }
 
@@ -633,10 +598,7 @@ int rdb200_resolve_flats_epsilon_f32(float *dem, int32_t w, int32_t h, float nod
   return resolve_flats_epsilon(Side::host, dem, w, h, nodata);
 }
 int rdb200_get_flat_mask_f32(const float *dem, int32_t *flat_mask, int32_t *labels, int32_t w, int32_t h, float nodata) {
-  return raster_call(Side::host, "get_flat_mask: null pointer", {dem, flat_mask, labels}, w, h, [&](Arrays &a, size_t n) {
-    // the staged copy of dem is not written: apply is false
-    resolve_flats_dev(const_cast<float *>(a.in(dem, n)), w, h, nodata, a.out(flat_mask, n), a.out(labels, n), false);
-  });
+  return get_flat_mask(Side::host, dem, flat_mask, labels, w, h, nodata);
 }
 int rdb200_d8_flow_directions_f32(const float *dem, uint8_t *dirs, int32_t w, int32_t h, float nodata) {
   return d8_flow_directions(Side::host, dem, dirs, w, h, nodata);
@@ -691,71 +653,71 @@ int rdb200_fa_tarboton_f32_f64(const float *dem, double *accum, int32_t w, int32
   return fa_fused(Side::host, dem, accum, w, h, nodata, ones, true);
 }
 
-int rdb200_fill_depressions_d8_f64(double *dem, int32_t w, int32_t h) { return fill_depressions_f64(Side::host, dem, w, h, false); }
-int rdb200_fill_depressions_d4_f64(double *dem, int32_t w, int32_t h) { return fill_depressions_f64(Side::host, dem, w, h, true); }
+int rdb200_fill_depressions_d8_f64(double *dem, int32_t w, int32_t h) { return fill_depressions(Side::host, dem, w, h, false); }
+int rdb200_fill_depressions_d4_f64(double *dem, int32_t w, int32_t h) { return fill_depressions(Side::host, dem, w, h, true); }
 int rdb200_pit_mask_d8_f64(const double *dem, uint8_t *mask, int32_t w, int32_t h, double nodata) {
-  return pit_mask_f64(Side::host, dem, mask, w, h, nodata, false);
+  return pit_mask(Side::host, dem, mask, w, h, nodata, false);
 }
 int rdb200_pit_mask_d4_f64(const double *dem, uint8_t *mask, int32_t w, int32_t h, double nodata) {
-  return pit_mask_f64(Side::host, dem, mask, w, h, nodata, true);
+  return pit_mask(Side::host, dem, mask, w, h, nodata, true);
 }
 int rdb200_has_depressions_d8_f64(const double *dem, int32_t w, int32_t h, int32_t *out) {
-  return has_depressions_f64(Side::host, dem, w, h, out, false);
+  return has_depressions(Side::host, dem, w, h, out, false);
 }
 int rdb200_has_depressions_d4_f64(const double *dem, int32_t w, int32_t h, int32_t *out) {
-  return has_depressions_f64(Side::host, dem, w, h, out, true);
+  return has_depressions(Side::host, dem, w, h, out, true);
 }
 int rdb200_resolve_flats_epsilon_f64(double *dem, int32_t w, int32_t h, double nodata) {
-  return resolve_flats_epsilon_f64(Side::host, dem, w, h, nodata);
+  return resolve_flats_epsilon(Side::host, dem, w, h, nodata);
 }
 int rdb200_d8_flow_directions_f64(const double *dem, uint8_t *dirs, int32_t w, int32_t h, double nodata) {
-  return d8_flow_directions_f64(Side::host, dem, dirs, w, h, nodata);
+  return d8_flow_directions(Side::host, dem, dirs, w, h, nodata);
 }
 int rdb200_get_flat_mask_f64(const double *dem, int32_t *flat_mask, int32_t *labels, int32_t w, int32_t h, double nodata) {
-  return get_flat_mask_f64(Side::host, dem, flat_mask, labels, w, h, nodata);
+  return get_flat_mask(Side::host, dem, flat_mask, labels, w, h, nodata);
 }
 int rdb200_d8_flow_directions_flats_f64(double *dem, uint8_t *dirs, int32_t w, int32_t h, double nodata, int32_t alter) {
-  return d8_flow_directions_flats_f64(Side::host, dem, dirs, w, h, nodata, alter);
+  return d8_flow_directions_flats(Side::host, dem, dirs, w, h, nodata, alter);
 }
 int rdb200_fa_d8_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata, int32_t ones) {
-  return fa_d8_f64(Side::host, dem, accum, w, h, nodata, ones);
+  return fa_fused(Side::host, dem, accum, w, h, nodata, ones, false);
 }
 int rdb200_fa_d4_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata) {
-  return fa_d4_f64(Side::host, dem, accum, w, h, nodata);
+  return fa_via_props(Side::host, 2, dem, accum, w, h, nodata, 0);
 }
 int rdb200_fm_d8_f64(const double *dem, float *props, int32_t w, int32_t h, double nodata) {
-  return fm_f64(Side::host, 0, dem, props, w, h, nodata);
+  return fm(Side::host, 0, dem, props, w, h, nodata);
 }
 int rdb200_fm_tarboton_f64(const double *dem, float *props, int32_t w, int32_t h, double nodata) {
-  return fm_f64(Side::host, 1, dem, props, w, h, nodata);
+  return fm(Side::host, 1, dem, props, w, h, nodata);
 }
 int rdb200_fm_d4_f64(const double *dem, float *props, int32_t w, int32_t h, double nodata) {
-  return fm_f64(Side::host, 2, dem, props, w, h, nodata);
+  return fm(Side::host, 2, dem, props, w, h, nodata);
 }
 int rdb200_fm_quinn_f64(const double *dem, float *props, int32_t w, int32_t h, double nodata) {
-  return fm_f64(Side::host, 3, dem, props, w, h, nodata, 1.0);
+  return fm(Side::host, 3, dem, props, w, h, nodata, 1.0);
 }
 int rdb200_fm_holmgren_f64(const double *dem, float *props, int32_t w, int32_t h, double nodata, double xparam) {
-  return fm_f64(Side::host, 3, dem, props, w, h, nodata, xparam);
+  return fm(Side::host, 3, dem, props, w, h, nodata, xparam);
 }
 int rdb200_fm_freeman_f64(const double *dem, float *props, int32_t w, int32_t h, double nodata, double xparam) {
-  return fm_f64(Side::host, 4, dem, props, w, h, nodata, xparam);
+  return fm(Side::host, 4, dem, props, w, h, nodata, xparam);
 }
 int rdb200_fa_quinn_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata) {
-  return fa_method_f64(Side::host, 3, dem, accum, w, h, nodata, 1.0);
+  return fa_via_props(Side::host, 3, dem, accum, w, h, nodata, 1.0);
 }
 int rdb200_fa_holmgren_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata, double xparam) {
-  return fa_method_f64(Side::host, 3, dem, accum, w, h, nodata, xparam);
+  return fa_via_props(Side::host, 3, dem, accum, w, h, nodata, xparam);
 }
 int rdb200_fa_freeman_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata, double xparam) {
-  return fa_method_f64(Side::host, 4, dem, accum, w, h, nodata, xparam);
+  return fa_via_props(Side::host, 4, dem, accum, w, h, nodata, xparam);
 }
 int rdb200_fa_tarboton_f64_f64(const double *dem, double *accum, int32_t w, int32_t h, double nodata, int32_t ones) {
-  return fa_tarboton_f64(Side::host, dem, accum, w, h, nodata, ones);
+  return fa_fused(Side::host, dem, accum, w, h, nodata, ones, true);
 }
 int rdb200_terrain_attribute_f64(int32_t attribute, const double *dem, float *out, int32_t w, int32_t h, double nodata_in,
                                  float nodata_out, float zscale, double cell_x, double cell_y) {
-  return terrain_attribute_f64(Side::host, attribute, dem, out, w, h, nodata_in, nodata_out, zscale, cell_x, cell_y);
+  return terrain_attribute(Side::host, attribute, dem, out, w, h, nodata_in, nodata_out, zscale, cell_x, cell_y);
 }
 int rdb200_f64_order_keys(const double *dem, float *keys, int32_t w, int32_t h, double nodata, float *nodata_key,
                           int32_t *ranked) {
@@ -823,52 +785,52 @@ int rdb200_dev_terrain_attribute_f32(int32_t attribute, const float *d_dem, floa
 }
 
 int rdb200_dev_fill_depressions_d8_f64(double *d_dem, int32_t w, int32_t h) {
-  return fill_depressions_f64(Side::device, d_dem, w, h, false);
+  return fill_depressions(Side::device, d_dem, w, h, false);
 }
 int rdb200_dev_fill_depressions_d4_f64(double *d_dem, int32_t w, int32_t h) {
-  return fill_depressions_f64(Side::device, d_dem, w, h, true);
+  return fill_depressions(Side::device, d_dem, w, h, true);
 }
 int rdb200_dev_pit_mask_d8_f64(const double *d_dem, uint8_t *d_mask, int32_t w, int32_t h, double nodata) {
-  return pit_mask_f64(Side::device, d_dem, d_mask, w, h, nodata, false);
+  return pit_mask(Side::device, d_dem, d_mask, w, h, nodata, false);
 }
 int rdb200_dev_pit_mask_d4_f64(const double *d_dem, uint8_t *d_mask, int32_t w, int32_t h, double nodata) {
-  return pit_mask_f64(Side::device, d_dem, d_mask, w, h, nodata, true);
+  return pit_mask(Side::device, d_dem, d_mask, w, h, nodata, true);
 }
 int rdb200_dev_has_depressions_d8_f64(const double *d_dem, int32_t w, int32_t h, int32_t *out) {
-  return has_depressions_f64(Side::device, d_dem, w, h, out, false);
+  return has_depressions(Side::device, d_dem, w, h, out, false);
 }
 int rdb200_dev_has_depressions_d4_f64(const double *d_dem, int32_t w, int32_t h, int32_t *out) {
-  return has_depressions_f64(Side::device, d_dem, w, h, out, true);
+  return has_depressions(Side::device, d_dem, w, h, out, true);
 }
 int rdb200_dev_resolve_flats_epsilon_f64(double *d_dem, int32_t w, int32_t h, double nodata) {
-  return resolve_flats_epsilon_f64(Side::device, d_dem, w, h, nodata);
+  return resolve_flats_epsilon(Side::device, d_dem, w, h, nodata);
 }
 int rdb200_dev_d8_flow_directions_f64(const double *d_dem, uint8_t *d_dirs, int32_t w, int32_t h, double nodata) {
-  return d8_flow_directions_f64(Side::device, d_dem, d_dirs, w, h, nodata);
+  return d8_flow_directions(Side::device, d_dem, d_dirs, w, h, nodata);
 }
 int rdb200_dev_d8_flow_directions_flats_f64(double *d_dem, uint8_t *d_dirs, int32_t w, int32_t h, double nodata, int32_t alter) {
-  return d8_flow_directions_flats_f64(Side::device, d_dem, d_dirs, w, h, nodata, alter);
+  return d8_flow_directions_flats(Side::device, d_dem, d_dirs, w, h, nodata, alter);
 }
 int rdb200_dev_fa_d8_f64_f64(const double *d_dem, double *d_accum, int32_t w, int32_t h, double nodata, int32_t ones) {
-  return fa_d8_f64(Side::device, d_dem, d_accum, w, h, nodata, ones);
+  return fa_fused(Side::device, d_dem, d_accum, w, h, nodata, ones, false);
 }
 int rdb200_dev_fa_d4_f64_f64(const double *d_dem, double *d_accum, int32_t w, int32_t h, double nodata) {
-  return fa_d4_f64(Side::device, d_dem, d_accum, w, h, nodata);
+  return fa_via_props(Side::device, 2, d_dem, d_accum, w, h, nodata, 0);
 }
 int rdb200_dev_fm_method_f64(int32_t method, const double *d_dem, float *d_props, int32_t w, int32_t h, double nodata,
                              double xparam) {
-  return fm_f64(Side::device, method, d_dem, d_props, w, h, nodata, xparam);
+  return fm(Side::device, method, d_dem, d_props, w, h, nodata, xparam);
 }
 int rdb200_dev_fa_method_f64_f64(int32_t method, const double *d_dem, double *d_accum, int32_t w, int32_t h, double nodata,
                                  double xparam) {
-  return fa_method_f64(Side::device, method, d_dem, d_accum, w, h, nodata, xparam);
+  return fa_via_props(Side::device, method, d_dem, d_accum, w, h, nodata, xparam);
 }
 int rdb200_dev_fa_tarboton_f64_f64(const double *d_dem, double *d_accum, int32_t w, int32_t h, double nodata, int32_t ones) {
-  return fa_tarboton_f64(Side::device, d_dem, d_accum, w, h, nodata, ones);
+  return fa_fused(Side::device, d_dem, d_accum, w, h, nodata, ones, true);
 }
 int rdb200_dev_terrain_attribute_f64(int32_t attribute, const double *d_dem, float *d_out, int32_t w, int32_t h,
                                      double nodata_in, float nodata_out, float zscale, double cell_x, double cell_y) {
-  return terrain_attribute_f64(Side::device, attribute, d_dem, d_out, w, h, nodata_in, nodata_out, zscale, cell_x, cell_y);
+  return terrain_attribute(Side::device, attribute, d_dem, d_out, w, h, nodata_in, nodata_out, zscale, cell_x, cell_y);
 }
 int rdb200_dev_f64_order_keys(const double *d_dem, float *d_keys, int32_t w, int32_t h, double nodata, float *nodata_key,
                               int32_t *ranked) {
@@ -912,51 +874,23 @@ int rdb200_mgpu_has_depressions_d4_f32(const rdb200_comm *comm, const float *d_b
 int rdb200_mgpu_fa_method_f32_f64(const rdb200_comm *comm, const float *d_dem, double *d_accum, int32_t w, int32_t rows,
                                   float nodata, int32_t gt, int32_t gb, int32_t method, double xparam, int32_t ones,
                                   int32_t *exchange_rounds) {
-  int xr = 0;
-  const int rc = raster_call(Side::device, "mgpu_fa: null pointer", {d_dem, d_accum}, w, rows, [&](Arrays &, size_t) {
-    mgpu_fa_band(comm, d_dem, d_accum, w, rows, nodata, gt, gb, method, xparam, ones != 0, &xr);
-  });
-  if (rc == 0 && exchange_rounds) *exchange_rounds = xr;
-  return rc;
+  return mgpu_fa_method(comm, d_dem, d_accum, w, rows, nodata, gt, gb, method, xparam, ones, exchange_rounds);
 }
 int rdb200_mgpu_fa_f32_f64(const rdb200_comm *comm, const float *d_dem, double *d_accum, int32_t w, int32_t rows, float nodata,
                            int32_t gt, int32_t gb, int32_t dinf, int32_t ones, int32_t *exchange_rounds) {
   return rdb200_mgpu_fa_method_f32_f64(comm, d_dem, d_accum, w, rows, nodata, gt, gb, dinf ? 1 : 0, 0.0, ones, exchange_rounds);
 }
 
-// FM_x and TA_x over row bands: one exchange of the DEM's edge rows gives every owned cell its whole 3 x 3 neighbourhood,
-// and a local edge row is a raster edge row exactly when it is not a ghost row, so the single-GPU kernel on the local raster
-// gives the owned rows the single-GPU bits.
 int rdb200_mgpu_fm_method_f32(const rdb200_comm *comm, int32_t method, float *d_band_dem, float *d_band_props9, int32_t w,
                               int32_t rows, float nodata, int32_t gt, int32_t gb, double xparam) {
-  return raster_call(
-      Side::device, "mgpu_fm_method: null pointer", {d_band_props9, comm, d_band_dem}, w, rows,
-      [&] {
-        check_band_args("mgpu_fm_method", comm, d_band_dem, w, rows, gt, gb);
-        if (method < 0 || method > 4) fail("unknown flow metric %d", method);
-      },
-      [&](Arrays &, size_t) {
-        exchange_band_rows(comm, d_band_dem, sizeof(float), w, rows, gt, gb);
-        fm_dispatch_dev(method, d_band_dem, d_band_props9, w, rows, nodata, xparam);
-      });
+  return mgpu_fm_method(comm, method, d_band_dem, d_band_props9, w, rows, nodata, gt, gb, xparam);
 }
 
 int rdb200_mgpu_terrain_attribute_f32(const rdb200_comm *comm, int32_t attribute, float *d_band_dem, float *d_band_out, int32_t w,
                                       int32_t rows, float nodata_in, float nodata_out, float zscale, double cell_x, double cell_y,
                                       int32_t gt, int32_t gb) {
-  return raster_call(
-      Side::device, "mgpu_terrain_attribute: null pointer", {d_band_out, comm, d_band_dem}, w, rows,
-      [&] {
-        check_band_args("mgpu_terrain_attribute", comm, d_band_dem, w, rows, gt, gb);
-        if (attribute < RDB200_TA_SLOPE_RISERUN || attribute > RDB200_TA_PROFILE_CURVATURE)
-          fail("unknown terrain attribute %d", attribute);
-        if (!(cell_x > 0) || !(cell_y > 0))
-          fail("terrain attribute: cell lengths must be positive (got %g x %g)", cell_x, cell_y);
-      },
-      [&](Arrays &, size_t) {
-        exchange_band_rows(comm, d_band_dem, sizeof(float), w, rows, gt, gb);
-        terrain_attribute_dev(attribute, d_band_dem, d_band_out, w, rows, nodata_in, nodata_out, zscale, cell_x, cell_y);
-      });
+  return mgpu_terrain_attribute(comm, attribute, d_band_dem, d_band_out, w, rows, nodata_in, nodata_out, zscale, cell_x,
+                                cell_y, gt, gb);
 }
 
 int rdb200_mgpu_flow_accumulation_props_f64(const rdb200_comm *comm, float *d_band_props9, double *d_band_accum_inout, int32_t w,
@@ -972,24 +906,13 @@ int rdb200_mgpu_flow_accumulation_props_f64(const rdb200_comm *comm, float *d_ba
 
 int rdb200_mgpu_resolve_flats_epsilon_f32(const rdb200_comm *comm, float *d_band, int32_t w, int32_t rows, float nodata,
                                           int32_t gt, int32_t gb, int32_t *seam_iterations) {
-  int it = 0;
-  const int rc = raster_call(Side::device, "mgpu_resolve_flats: null pointer", {comm, d_band}, w, rows,
-                             [&](Arrays &, size_t) { mgpu_resolve_flats_band(comm, d_band, w, rows, nodata, gt, gb, &it); });
-  if (rc == 0 && seam_iterations) *seam_iterations = it;
-  return rc;
+  return mgpu_resolve_flats_epsilon(comm, d_band, w, rows, nodata, gt, gb, seam_iterations);
 }
 
 int rdb200_mgpu_d8_flow_directions_flats_f32(const rdb200_comm *comm, float *d_band_dem, uint8_t *d_band_dirs, int32_t w,
                                              int32_t rows, float nodata, int32_t gt, int32_t gb, int32_t alter,
                                              int32_t *seam_iterations) {
-  int it = 0;
-  const int rc = raster_call(Side::device, "mgpu_d8_flow_directions_flats: null pointer", {comm, d_band_dem, d_band_dirs}, w, rows,
-                             [&](Arrays &, size_t) {
-                               mgpu_d8_flow_directions_flats_band(comm, d_band_dem, d_band_dirs, w, rows, nodata, gt, gb,
-                                                                  alter != 0, &it);
-                             });
-  if (rc == 0 && seam_iterations) *seam_iterations = it;
-  return rc;
+  return mgpu_d8_flow_directions_flats(comm, d_band_dem, d_band_dirs, w, rows, nodata, gt, gb, alter, seam_iterations);
 }
 
 int rdb200_mgpu_d8_flow_accum_u8_i32(const rdb200_comm *comm, const uint8_t *d_band_dirs, int32_t *d_band_area, int32_t w,
@@ -1005,96 +928,56 @@ int rdb200_mgpu_d8_flow_accum_u8_i32(const rdb200_comm *comm, const uint8_t *d_b
 
 int rdb200_mgpu_fill_depressions_d8_f64(const rdb200_comm *comm, double *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb,
                                         int32_t row0, int32_t height, int32_t *exchange_rounds) {
-  return mgpu_fill_f64(comm, d_band, w, rows, gt, gb, row0, height, exchange_rounds, false);
+  return mgpu_fill(comm, d_band, w, rows, gt, gb, row0, height, exchange_rounds, false);
 }
 int rdb200_mgpu_fill_depressions_d4_f64(const rdb200_comm *comm, double *d_band, int32_t w, int32_t rows, int32_t gt, int32_t gb,
                                         int32_t row0, int32_t height, int32_t *exchange_rounds) {
-  return mgpu_fill_f64(comm, d_band, w, rows, gt, gb, row0, height, exchange_rounds, true);
+  return mgpu_fill(comm, d_band, w, rows, gt, gb, row0, height, exchange_rounds, true);
 }
 int rdb200_mgpu_pit_mask_d8_f64(const rdb200_comm *comm, const double *d_band, uint8_t *d_band_mask, int32_t w, int32_t rows,
                                 double nodata, int32_t gt, int32_t gb, int32_t row0, int32_t height) {
-  return mgpu_pit_mask_f64(comm, d_band, d_band_mask, w, rows, nodata, gt, gb, row0, height, false);
+  return mgpu_pit_mask(comm, d_band, d_band_mask, w, rows, nodata, gt, gb, row0, height, false);
 }
 int rdb200_mgpu_pit_mask_d4_f64(const rdb200_comm *comm, const double *d_band, uint8_t *d_band_mask, int32_t w, int32_t rows,
                                 double nodata, int32_t gt, int32_t gb, int32_t row0, int32_t height) {
-  return mgpu_pit_mask_f64(comm, d_band, d_band_mask, w, rows, nodata, gt, gb, row0, height, true);
+  return mgpu_pit_mask(comm, d_band, d_band_mask, w, rows, nodata, gt, gb, row0, height, true);
 }
 int rdb200_mgpu_has_depressions_d8_f64(const rdb200_comm *comm, const double *d_band, int32_t w, int32_t rows, int32_t gt,
                                        int32_t gb, int32_t row0, int32_t height, int32_t *out) {
-  return mgpu_has_depressions_f64(comm, d_band, w, rows, gt, gb, row0, height, out, false);
+  return mgpu_has_depressions(comm, d_band, w, rows, gt, gb, row0, height, out, false);
 }
 int rdb200_mgpu_has_depressions_d4_f64(const rdb200_comm *comm, const double *d_band, int32_t w, int32_t rows, int32_t gt,
                                        int32_t gb, int32_t row0, int32_t height, int32_t *out) {
-  return mgpu_has_depressions_f64(comm, d_band, w, rows, gt, gb, row0, height, out, true);
+  return mgpu_has_depressions(comm, d_band, w, rows, gt, gb, row0, height, out, true);
 }
 
 int rdb200_mgpu_resolve_flats_epsilon_f64(const rdb200_comm *comm, double *d_band, int32_t w, int32_t rows, double nodata,
                                           int32_t gt, int32_t gb, int32_t *seam_iterations) {
-  int it = 0;
-  const int rc = raster_call(Side::device, "mgpu_resolve_flats: null pointer", {comm, d_band}, w, rows,
-                             [&](Arrays &, size_t) { mgpu_resolve_flats_f64_band(comm, d_band, w, rows, nodata, gt, gb, &it); });
-  if (rc == 0 && seam_iterations) *seam_iterations = it;
-  return rc;
+  return mgpu_resolve_flats_epsilon(comm, d_band, w, rows, nodata, gt, gb, seam_iterations);
 }
 
 int rdb200_mgpu_d8_flow_directions_flats_f64(const rdb200_comm *comm, double *d_band_dem, uint8_t *d_band_dirs, int32_t w,
                                              int32_t rows, double nodata, int32_t gt, int32_t gb, int32_t alter,
                                              int32_t *seam_iterations) {
-  int it = 0;
-  const int rc = raster_call(Side::device, "mgpu_d8_flow_directions_flats: null pointer", {comm, d_band_dem, d_band_dirs}, w, rows,
-                             [&](Arrays &, size_t) {
-                               mgpu_d8_flow_directions_flats_f64_band(comm, d_band_dem, d_band_dirs, w, rows, nodata, gt, gb,
-                                                                      alter != 0, &it);
-                             });
-  if (rc == 0 && seam_iterations) *seam_iterations = it;
-  return rc;
+  return mgpu_d8_flow_directions_flats(comm, d_band_dem, d_band_dirs, w, rows, nodata, gt, gb, alter, seam_iterations);
 }
 
 int rdb200_mgpu_fm_method_f64(const rdb200_comm *comm, int32_t method, double *d_band_dem, float *d_band_props9, int32_t w,
                               int32_t rows, double nodata, int32_t gt, int32_t gb, double xparam) {
-  return raster_call(
-      Side::device, "mgpu_fm_method: null pointer", {d_band_props9, comm, d_band_dem}, w, rows,
-      [&] {
-        check_band_args("mgpu_fm_method", comm, d_band_dem, w, rows, gt, gb);
-        if (method < 0 || method > 4) fail("unknown flow metric %d", method);
-      },
-      [&](Arrays &, size_t) {
-        exchange_band_rows(comm, d_band_dem, sizeof(double), w, rows, gt, gb);
-        fm_method_f64_dev(method, d_band_dem, d_band_props9, w, rows, nodata, xparam);
-      });
+  return mgpu_fm_method(comm, method, d_band_dem, d_band_props9, w, rows, nodata, gt, gb, xparam);
 }
 
 int rdb200_mgpu_terrain_attribute_f64(const rdb200_comm *comm, int32_t attribute, double *d_band_dem, float *d_band_out, int32_t w,
                                       int32_t rows, double nodata_in, float nodata_out, float zscale, double cell_x, double cell_y,
                                       int32_t gt, int32_t gb) {
-  return raster_call(
-      Side::device, "mgpu_terrain_attribute: null pointer", {d_band_out, comm, d_band_dem}, w, rows,
-      [&] {
-        check_band_args("mgpu_terrain_attribute", comm, d_band_dem, w, rows, gt, gb);
-        if (attribute < RDB200_TA_SLOPE_RISERUN || attribute > RDB200_TA_PROFILE_CURVATURE)
-          fail("unknown terrain attribute %d", attribute);
-        if (!(cell_x > 0) || !(cell_y > 0))
-          fail("terrain attribute: cell lengths must be positive (got %g x %g)", cell_x, cell_y);
-      },
-      [&](Arrays &, size_t) {
-        exchange_band_rows(comm, d_band_dem, sizeof(double), w, rows, gt, gb);
-        terrain_attribute_f64_dev(attribute, d_band_dem, d_band_out, w, rows, nodata_in, nodata_out, zscale, cell_x, cell_y);
-      });
+  return mgpu_terrain_attribute(comm, attribute, d_band_dem, d_band_out, w, rows, nodata_in, nodata_out, zscale, cell_x,
+                                cell_y, gt, gb);
 }
 
 int rdb200_mgpu_fa_method_f64_f64(const rdb200_comm *comm, const double *d_dem, double *d_accum, int32_t w, int32_t rows,
                                   double nodata, int32_t gt, int32_t gb, int32_t method, double xparam, int32_t ones,
                                   int32_t *exchange_rounds) {
-  int xr = 0;
-  const int rc = raster_call(
-      Side::device, "mgpu_fa: null pointer", {comm, d_dem, d_accum}, w, rows,
-      [&] {
-        check_band_args("mgpu_fa", comm, d_dem, w, rows, gt, gb);
-        check_fa_method(method, xparam);
-      },
-      [&](Arrays &, size_t) { mgpu_fa_f64_band(comm, d_dem, d_accum, w, rows, nodata, gt, gb, method, xparam, ones != 0, &xr); });
-  if (rc == 0 && exchange_rounds) *exchange_rounds = xr;
-  return rc;
+  return mgpu_fa_method(comm, d_dem, d_accum, w, rows, nodata, gt, gb, method, xparam, ones, exchange_rounds);
 }
 
 int rdb200_mgpu_f64_order_keys(const rdb200_comm *comm, const double *d_band, float *d_band_keys, int32_t w, int32_t rows,

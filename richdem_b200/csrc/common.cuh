@@ -184,8 +184,12 @@ void check_band_args(const char *what, const rdb200_comm *comm, const void *d_ba
 void exchange_band_rows(const rdb200_comm *comm, void *d_band, size_t elem, int w, int hloc, int gt, int gb);
 void mgpu_fill_band(const rdb200_comm *comm, float *d_local, int w, int hloc, int gt, int gb, int row0, int H, int *xrounds,
                     bool topo4 = false);
+void mgpu_fill_band(const rdb200_comm *comm, double *d_band, int w, int hloc, int gt, int gb, int row0, int H, int *xrounds,
+                    bool topo4);
 // method: 0 D8, 1 Tarboton, 2 D4, 3 Holmgren (xparam; Quinn = 1.0), 4 Freeman (xparam)
 void mgpu_fa_band(const rdb200_comm *comm, const float *d_dem, double *d_accum, int w, int hloc, float nodata, int gt, int gb,
+                  int method, double xparam, bool ones, int *xrounds);
+void mgpu_fa_band(const rdb200_comm *comm, const double *d_dem, double *d_accum, int w, int hloc, double nodata, int gt, int gb,
                   int method, double xparam, bool ones, int *xrounds);
 void check_fa_method(int method, double xparam);  // an unknown method, or a non-finite exponent, is an error
 // FlowAccumulation(props, accum) of caller-supplied 9-float proportions; the ghost rows of d_props are overwritten with the
@@ -195,7 +199,11 @@ void mgpu_flow_accumulation_props_band(const rdb200_comm *comm, float *d_props, 
 // d_mask_out (w x hloc, may be null): write the increment mask there and leave the elevations and their ghost rows alone
 void mgpu_resolve_flats_band(const rdb200_comm *comm, float *d_local, int w, int hloc, float nodata, int gt, int gb,
                              int *seam_iters, int32_t *d_mask_out = nullptr);
+void mgpu_resolve_flats_band(const rdb200_comm *comm, double *d_band, int w, int hloc, double nodata, int gt, int gb,
+                             int *seam_iters);
 void mgpu_d8_flow_directions_flats_band(const rdb200_comm *comm, float *d_dem, uint8_t *d_dirs, int w, int hloc, float nodata,
+                                        int gt, int gb, bool alter, int *seam_iters);
+void mgpu_d8_flow_directions_flats_band(const rdb200_comm *comm, double *d_band, uint8_t *d_dirs, int w, int hloc, double nodata,
                                         int gt, int gb, bool alter, int *seam_iters);
 // the flats of a band's plain D8 directions resolved over the bands (barnes_flat_resolution_d8 between its two direction
 // passes); with alter, d_mask_out (may be null) receives the increment mask instead of d_dem its float ulps
@@ -207,7 +215,10 @@ void mgpu_d8_flow_accum_band(const rdb200_comm *comm, const uint8_t *d_dirs, int
 int mgpu_relax_band(const rdb200_comm *comm, rdb200_fill_state *state, int gt, int gb, int R);
 
 // ---- stage entry points implemented in the .cu files (device pointers, ctx stream) -------
+// A double overload runs the float engines on order-preserving float keys (f64.cu) where the stage only compares
+// elevations, and the kernels' double instantiations where it does arithmetic on them.
 void fill_depressions_dev(float *d_dem, int w, int h, bool topo4 = false);
+void fill_depressions_dev(double *d_z, int w, int h, bool topo4 = false);
 void geodesic_distance_dev(const uint8_t *d_open, int open_bit, float *d_w_inout, int w, int h);
 void geodesic_distance_pair_dev(const uint8_t *d_open, int open_bit, float *d_wa, float *d_wb, int w, int h);
 rdb200_fill_state *new_band_distance_state(const uint8_t *d_open, int open_bit, const float *d_winit, int w, int h,
@@ -215,54 +226,60 @@ rdb200_fill_state *new_band_distance_state(const uint8_t *d_open, int open_bit, 
 void finish_band_distance_state(rdb200_fill_state *s, float *d_out);
 void resolve_flats_dev(float *d_dem, int w, int h, float nodata, int32_t *d_mask_out,
                        int32_t *d_labels_out, bool apply, const uint8_t *d_dirs = nullptr);
+// ResolveFlatsEpsilon and GetFlatMask
+inline void resolve_flats_epsilon_dev(float *d_dem, int w, int h, float nodata) {
+  resolve_flats_dev(d_dem, w, h, nodata, nullptr, nullptr, true);
+}
+void resolve_flats_epsilon_dev(double *d_z, int w, int h, double nodata);
+inline void get_flat_mask_dev(const float *d_dem, int32_t *d_mask, int32_t *d_labels, int w, int h, float nodata) {
+  resolve_flats_dev(const_cast<float *>(d_dem), w, h, nodata, d_mask, d_labels, false);  // apply = false: d_dem is not written
+}
+void get_flat_mask_dev(const double *d_z, int32_t *d_mask, int32_t *d_labels, int w, int h, double nodata);
 void d8_flow_directions_flats_dev(float *d_dem, uint8_t *d_dirs, int w, int h, float nodata, bool alter);
+void d8_flow_directions_flats_dev(double *d_z, uint8_t *d_dirs, int w, int h, double nodata, bool alter);
 void d8_flow_directions_dev(const float *d_dem, uint8_t *d_dirs, int w, int h, float nodata);
+void d8_flow_directions_dev(const double *d_dem, uint8_t *d_dirs, int w, int h, double nodata);
 // d8_flow_flats: interior NO_FLOW cells take the direction of their lowest same-label neighbour in the increment mask
 void d8_flow_flats_dev(const int32_t *d_mask, const int32_t *d_labels, uint8_t *d_dirs, int w, int h);
 void d8_flow_accum_dev(const uint8_t *d_dirs, int32_t *d_area, int w, int h);
-void fm_d8_dev(const float *d_dem, float *d_props, int w, int h, float nodata);
-void fm_tarboton_dev(const float *d_dem, float *d_props, int w, int h, float nodata);
-void fm_d4_dev(const float *d_dem, float *d_props, int w, int h, float nodata);
-void fm_holmgren_dev(const float *d_dem, float *d_props, int w, int h, float nodata, double xparam);
-void fm_freeman_dev(const float *d_dem, float *d_props, int w, int h, float nodata, double xparam);
+// FM_x by the C ABI's method number: 0 FM_D8, 1 FM_Tarboton, 2 FM_D4, 3 FM_Holmgren (FM_Quinn = exponent 1), 4 FM_Freeman
+// (T = float, double)
+template <class T>
+void fm_method_dev(int method, const T *d_dem, float *d_props, int w, int h, T nodata, double xparam);
 void flow_accumulation_props_dev(const float *d_props, double *d_accum, int w, int h);
-void fa_fused_dev(const float *d_dem, double *d_accum, int w, int h, float nodata, bool ones,
-                  bool dinf);
+// FA_D8 (dinf false) / FA_Tarboton by the fused engines
+void fa_fused_dev(const float *d_dem, double *d_accum, int w, int h, float nodata, bool ones, bool dinf);
+void fa_fused_dev(const double *d_dem, double *d_accum, int w, int h, double nodata, bool ones, bool dinf);
 void terrain_attribute_dev(int attribute_id, const float *d_dem, float *d_out, int w, int h, float nodata_in, float nodata_out,
                            float zscale, double cell_x, double cell_y);
+void terrain_attribute_dev(int attribute_id, const double *d_dem, float *d_out, int w, int h, double nodata_in,
+                           float nodata_out, float zscale, double cell_x, double cell_y);
 void generate_fbm_dev(float *d_dem, int w, int h, int y0, uint32_t seed, int octaves, float quantum);
 // pit_mask<topo> / HasDepressions<topo> (depressions.cu); d_dem is not modified
 void pit_mask_dev(const float *d_dem, uint8_t *d_mask, int w, int h, float nodata, bool topo4);
+void pit_mask_dev(const double *d_z, uint8_t *d_mask, int w, int h, double nodata, bool topo4);
 bool has_depressions_dev(const float *d_dem, int w, int h, bool topo4);
+bool has_depressions_dev(const double *d_z, int w, int h, bool topo4);
 void mgpu_pit_mask_band(const rdb200_comm *comm, const float *d_band, uint8_t *d_mask, int w, int hloc, float nodata, int gt,
+                        int gb, int row0, int H, bool topo4);
+void mgpu_pit_mask_band(const rdb200_comm *comm, const double *d_band, uint8_t *d_mask, int w, int hloc, double nodata, int gt,
                         int gb, int row0, int H, bool topo4);
 bool mgpu_has_depressions_band(const rdb200_comm *comm, const float *d_band, int w, int hloc, int gt, int gb, int row0, int H,
                                bool topo4);
-// pit_mask's compare pass (mask may be null) and the strict-pit stencil, OR-ed into the device flags
+bool mgpu_has_depressions_band(const rdb200_comm *comm, const double *d_band, int w, int hloc, int gt, int gb, int row0, int H,
+                               bool topo4);
+// pit_mask's compare pass (mask may be null) and the strict-pit stencil (T = float, double), OR-ed into the device flags
 void pit_mask_compare_dev(const float *d_z, const float *d_l, uint8_t *d_mask, size_t n, float nodata, int *d_any);
-void strict_pit_f64_dev(const double *d_z, int w, int h, bool topo4, int *d_flag);
-void d8_flow_directions_f64_dev(const double *d_dem, uint8_t *d_dirs, int w, int h, double nodata);
+template <class T>
+void strict_pit_dev(const T *d_z, int w, int h, bool topo4, int *d_flag);
 
 // ---- float64 rasters through order-preserving float keys (f64.cu) ---------------------------
 // kappa(Z) of n doubles into d_key; returns kappa(nodata).  *ranked (may be null): 0 when kappa is the cast to float,
 // 1 when it is the dense rank.  With table, case 2 allocates the kappa^-1 table of sorted distinct values (n doubles).
 float f64_keys_dev(const double *d_z, float *d_key, size_t n, double nodata, DevBuf<double> *table, int *ranked);
-void fill_depressions_f64_dev(double *d_z, int w, int h, bool topo4);
-void pit_mask_f64_dev(const double *d_z, uint8_t *d_mask, int w, int h, double nodata, bool topo4);
-bool has_depressions_f64_dev(const double *d_z, int w, int h, bool topo4);
-void resolve_flats_f64_dev(double *d_z, int w, int h, double nodata);
-void fa_d8_f64_dev(const double *d_z, double *d_accum, int w, int h, double nodata, bool ones);
-// D-infinity, MFD and terrain attributes on doubles: the float kernels' double instantiations (flowdirs.cu, accum.cu,
-// attributes.cu), no keys -- these stages do arithmetic on the elevations
-void fm_method_f64_dev(int method, const double *d_dem, float *d_props, int w, int h, double nodata, double xparam);
-void fa_tarboton_f64_dev(const double *d_dem, double *d_accum, int w, int h, double nodata, bool ones);
-void terrain_attribute_f64_dev(int attribute_id, const double *d_dem, float *d_out, int w, int h, double nodata_in,
-                               float nodata_out, float zscale, double cell_x, double cell_y);
 void f64_apply_ulps_dev(double *d_z, const int32_t *d_mask, int w, int h);
 // d8_flats_alter_dem on doubles: the reference's nextafterf, i.e. k float ulps of the double rounded to float
 void f64_float_steps_dev(double *d_z, const int32_t *d_mask, int w, int h);
-void get_flat_mask_f64_dev(const double *d_z, int32_t *d_mask, int32_t *d_labels, int w, int h, double nodata);
-void d8_flow_directions_flats_f64_dev(double *d_z, uint8_t *d_dirs, int w, int h, double nodata, bool alter);
 int32_t read_i32(const int32_t *d_value);  // one device int, read back after the library's stream
 
 // ---- float64 row bands: kappa_G, one key map shared by every band (f64.cu), and the band drivers (f64_band.cu) ----
@@ -283,17 +300,5 @@ void mgpu_f64_writeback_dev(const rdb200_comm *comm, const BandKeys &inv, double
                             int hloc, int gt, int gb);
 void check_mask_band(const char *what, const rdb200_comm *comm, const void *d_band, int w, int hloc, int gt, int gb, int row0,
                      int H);
-void mgpu_fill_f64_band(const rdb200_comm *comm, double *d_band, int w, int hloc, int gt, int gb, int row0, int H, int *xrounds,
-                        bool topo4);
-void mgpu_pit_mask_f64_band(const rdb200_comm *comm, const double *d_band, uint8_t *d_mask, int w, int hloc, double nodata, int gt,
-                            int gb, int row0, int H, bool topo4);
-bool mgpu_has_depressions_f64_band(const rdb200_comm *comm, const double *d_band, int w, int hloc, int gt, int gb, int row0, int H,
-                                   bool topo4);
-void mgpu_resolve_flats_f64_band(const rdb200_comm *comm, double *d_band, int w, int hloc, double nodata, int gt, int gb,
-                                 int *seam_iters);
-void mgpu_d8_flow_directions_flats_f64_band(const rdb200_comm *comm, double *d_band, uint8_t *d_dirs, int w, int hloc, double nodata,
-                                            int gt, int gb, bool alter, int *seam_iters);
-void mgpu_fa_f64_band(const rdb200_comm *comm, const double *d_dem, double *d_accum, int w, int hloc, double nodata, int gt, int gb,
-                      int method, double xparam, bool ones, int *xrounds);
 
 }  // namespace rdb

@@ -121,7 +121,7 @@ void pit_mask_compare_dev(const float *d_z, const float *d_l, uint8_t *d_mask, s
 
 // strict-pit pass over a w x h raster whose first and last rows and columns are not tested; OR-ed into *d_flag
 template <class T>
-static void strict_pit_launch(const T *d_z, int w, int h, bool topo4, int *d_flag) {
+void strict_pit_dev(const T *d_z, int w, int h, bool topo4, int *d_flag) {
   Ctx &c = ctx();
   if (w < 3 || h < 3) return;
   const int strips = (h - 2 + PIT_ROWS - 1) / PIT_ROWS;
@@ -131,10 +131,8 @@ static void strict_pit_launch(const T *d_z, int w, int h, bool topo4, int *d_fla
   RDB_CK(cudaGetLastError());
   count_launch();
 }
-void strict_pit_dev(const float *d_z, int w, int h, bool topo4, int *d_flag) { strict_pit_launch(d_z, w, h, topo4, d_flag); }
-void strict_pit_f64_dev(const double *d_z, int w, int h, bool topo4, int *d_flag) {
-  strict_pit_launch(d_z, w, h, topo4, d_flag);
-}
+template void strict_pit_dev(const float *, int, int, bool, int *);
+template void strict_pit_dev(const double *, int, int, bool, int *);
 
 // L = the fill of d_dem, in a scratch copy (the fill relaxes its water surface in the raster it is handed)
 static void fill_copy_dev(const float *d_dem, float *d_l, int w, int h, bool topo4) {
@@ -153,19 +151,47 @@ void pit_mask_dev(const float *d_dem, uint8_t *d_mask, int w, int h, float nodat
   ctx().stats.cells = (int64_t)n;
 }
 
-bool has_depressions_dev(const float *d_dem, int w, int h, bool topo4) {
-  Ctx &c = ctx();
+// pit_mask of a double raster: pit_mask of its keys, with kappa(nodata)
+void pit_mask_dev(const double *d_z, uint8_t *d_mask, int w, int h, double nodata, bool topo4) {
   const size_t n = (size_t)w * h;
-  DevBuf<int> flag(1);
-  RDB_CK(cudaMemsetAsync(flag.p, 0, sizeof(int), c.stream));
-  strict_pit_dev(d_dem, w, h, topo4, flag.p);
-  if (read_flag(flag.p)) return true;
-  if (w < 3 || h < 3) return false;  // every cell is an edge cell
+  DevBuf<float> key(n);
+  const float nd = f64_keys_dev(d_z, key.p, n, nodata, nullptr, nullptr);
+  pit_mask_dev(key.p, d_mask, w, h, nd, topo4);
+}
+
+// the strict-pit pass on d_z into a zeroed *d_flag: a strict pit answers HasDepressions alone
+template <class T>
+static bool strict_pit_found(const T *d_z, int w, int h, bool topo4, int *d_flag) {
+  RDB_CK(cudaMemsetAsync(d_flag, 0, sizeof(int), ctx().stream));
+  strict_pit_dev(d_z, w, h, topo4, d_flag);
+  return read_flag(d_flag) != 0;
+}
+
+// HasDepressions when no strict pit was found: whether the fill of d_dem raises a cell (OR-ed into *d_flag)
+static bool fill_raises(const float *d_dem, int w, int h, bool topo4, int *d_flag) {
+  const size_t n = (size_t)w * h;
   DevBuf<float> l(n);
   fill_copy_dev(d_dem, l.p, w, h, topo4);
-  pit_mask_compare_dev(d_dem, l.p, nullptr, n, 0.f, flag.p);
-  c.stats.cells = (int64_t)n;
-  return read_flag(flag.p) != 0;
+  pit_mask_compare_dev(d_dem, l.p, nullptr, n, 0.f, d_flag);
+  ctx().stats.cells = (int64_t)n;
+  return read_flag(d_flag) != 0;
+}
+
+bool has_depressions_dev(const float *d_dem, int w, int h, bool topo4) {
+  DevBuf<int> flag(1);
+  if (strict_pit_found(d_dem, w, h, topo4, flag.p)) return true;
+  if (w < 3 || h < 3) return false;  // every cell is an edge cell
+  return fill_raises(d_dem, w, h, topo4, flag.p);
+}
+
+// HasDepressions of a double raster: strict pits of the doubles (no keys needed), then the fill of the keys
+bool has_depressions_dev(const double *d_z, int w, int h, bool topo4) {
+  DevBuf<int> flag(1);
+  if (strict_pit_found(d_z, w, h, topo4, flag.p)) return true;
+  if (w < 3 || h < 3) return false;
+  DevBuf<float> key((size_t)w * h);
+  f64_keys_dev(d_z, key.p, (size_t)w * h, 0.0, nullptr, nullptr);
+  return fill_raises(key.p, w, h, topo4, flag.p);
 }
 
 // ---- row bands ---------------------------------------------------------------------------------------------------

@@ -530,7 +530,7 @@ float f64_keys_dev(const double *d_z, float *d_key, size_t n, double nodata, Dev
 }
 
 // FillDepressions<D8 / D4> of a double raster: fill the key raster, then write kappa^-1 of every raised key
-void fill_depressions_f64_dev(double *d_z, int w, int h, bool topo4) {
+void fill_depressions_dev(double *d_z, int w, int h, bool topo4) {
   Ctx &c = ctx();
   const size_t n = (size_t)w * h;
   DevBuf<float> k0(n), kf(n);
@@ -544,43 +544,8 @@ void fill_depressions_f64_dev(double *d_z, int w, int h, bool topo4) {
   c.stats.cells = (int64_t)n;
 }
 
-void pit_mask_f64_dev(const double *d_z, uint8_t *d_mask, int w, int h, double nodata, bool topo4) {
-  Ctx &c = ctx();
-  const size_t n = (size_t)w * h;
-  DevBuf<float> k0(n), kf(n);
-  DevBuf<int> any(1);
-  const float nd = f64_keys_dev(d_z, k0.p, n, nodata, nullptr, nullptr);
-  RDB_CK(cudaMemsetAsync(any.p, 0, sizeof(int), c.stream));
-  RDB_CK(cudaMemcpyAsync(kf.p, k0.p, n * sizeof(float), cudaMemcpyDeviceToDevice, c.stream));
-  fill_depressions_dev(kf.p, w, h, topo4);
-  pit_mask_compare_dev(k0.p, kf.p, d_mask, n, nd, any.p);
-  c.stats.cells = (int64_t)n;
-}
-
-bool has_depressions_f64_dev(const double *d_z, int w, int h, bool topo4) {
-  Ctx &c = ctx();
-  const size_t n = (size_t)w * h;
-  DevBuf<int> flag(1);
-  RDB_CK(cudaMemsetAsync(flag.p, 0, sizeof(int), c.stream));
-  strict_pit_f64_dev(d_z, w, h, topo4, flag.p);
-  int *hf = (int *)c.pinned;
-  RDB_CK(cudaMemcpyAsync(hf, flag.p, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-  RDB_CK(cudaStreamSynchronize(c.stream));
-  if (*hf) return true;
-  if (w < 3 || h < 3) return false;  // every cell is an edge cell
-  DevBuf<float> k0(n), kf(n);
-  f64_keys_dev(d_z, k0.p, n, 0.0, nullptr, nullptr);
-  RDB_CK(cudaMemcpyAsync(kf.p, k0.p, n * sizeof(float), cudaMemcpyDeviceToDevice, c.stream));
-  fill_depressions_dev(kf.p, w, h, topo4);
-  pit_mask_compare_dev(k0.p, kf.p, nullptr, n, 0.f, flag.p);
-  RDB_CK(cudaMemcpyAsync(hf, flag.p, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-  RDB_CK(cudaStreamSynchronize(c.stream));
-  c.stats.cells = (int64_t)n;
-  return *hf != 0;
-}
-
 // ResolveFlatsEpsilon: the increment mask of the key raster (GetFlatMask), applied as double ulps to the original values
-void resolve_flats_f64_dev(double *d_z, int w, int h, double nodata) {
+void resolve_flats_epsilon_dev(double *d_z, int w, int h, double nodata) {
   Ctx &c = ctx();
   const size_t n = (size_t)w * h;
   DevBuf<float> key(n);
@@ -593,20 +558,20 @@ void resolve_flats_f64_dev(double *d_z, int w, int h, double nodata) {
 }
 
 // GetFlatMask<double>: the increment mask and labels of the key raster (the flats compare elevations only)
-void get_flat_mask_f64_dev(const double *d_z, int32_t *d_mask, int32_t *d_labels, int w, int h, double nodata) {
+void get_flat_mask_dev(const double *d_z, int32_t *d_mask, int32_t *d_labels, int w, int h, double nodata) {
   const size_t n = (size_t)w * h;
   DevBuf<float> key(n);
   const float nd = f64_keys_dev(d_z, key.p, n, nodata, nullptr, nullptr);
-  resolve_flats_dev(key.p, w, h, nd, d_mask, d_labels, false);
+  get_flat_mask_dev(key.p, d_mask, d_labels, w, h, nd);
 }
 
 // barnes_flat_resolution_d8<double, uint8_t> (flats/flat_resolution.hpp:588-607): D8 directions of the doubles, then the
 // increment mask and labels of the flats the direction grid shows, on the keys (flats_from_dirs_kernel compares with ==
 // and < only), then either d8_flow_flats or d8_flats_alter_dem's float steps on the doubles and their directions again
-void d8_flow_directions_flats_f64_dev(double *d_z, uint8_t *d_dirs, int w, int h, double nodata, bool alter) {
+void d8_flow_directions_flats_dev(double *d_z, uint8_t *d_dirs, int w, int h, double nodata, bool alter) {
   Ctx &c = ctx();
   const size_t n = (size_t)w * h;
-  d8_flow_directions_f64_dev(d_z, d_dirs, w, h, nodata);
+  d8_flow_directions_dev(d_z, d_dirs, w, h, nodata);
   DevBuf<float> key(n);
   const float nd = f64_keys_dev(d_z, key.p, n, nodata, nullptr, nullptr);
   DevBuf<int32_t> mask(n), labels(alter ? 0 : n);
@@ -614,19 +579,11 @@ void d8_flow_directions_flats_f64_dev(double *d_z, uint8_t *d_dirs, int w, int h
   key.reset();
   if (alter) {
     f64_float_steps_dev(d_z, mask.p, w, h);
-    d8_flow_directions_f64_dev(d_z, d_dirs, w, h, nodata);
+    d8_flow_directions_dev(d_z, d_dirs, w, h, nodata);
   } else {
     d8_flow_flats_dev(mask.p, labels.p, d_dirs, w, h);
   }
   RDB_CK(cudaStreamSynchronize(c.stream));
-}
-
-// FA_D8 (unit or given weights) on the key raster: the accumulation carries no elevation values
-void fa_d8_f64_dev(const double *d_z, double *d_accum, int w, int h, double nodata, bool ones) {
-  const size_t n = (size_t)w * h;
-  DevBuf<float> key(n);
-  const float nd = f64_keys_dev(d_z, key.p, n, nodata, nullptr, nullptr);
-  fa_fused_dev(key.p, d_accum, w, h, nd, ones, false);
 }
 
 // ---- kappa_G: one key map for a raster cut into row bands (DESIGN §0.1 "kappa over row bands") ---------------------

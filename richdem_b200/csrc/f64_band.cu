@@ -27,8 +27,8 @@ void check_fill_band(const rdb200_comm *comm, const double *d_band, int w, int h
 
 // FillDepressions<D8 / D4>: kappa_G, the float32 band fill on the keys, kappa_G^-1 of the owned rows, and one exchange
 // so that the ghost rows hold the neighbours' filled edge rows, as the float32 band fill leaves them
-void mgpu_fill_f64_band(const rdb200_comm *comm, double *d_band, int w, int hloc, int gt, int gb, int row0, int H, int *xrounds,
-                        bool topo4) {
+void mgpu_fill_band(const rdb200_comm *comm, double *d_band, int w, int hloc, int gt, int gb, int row0, int H, int *xrounds,
+                    bool topo4) {
   check_fill_band(comm, d_band, w, hloc, gt, gb, row0, H);
   Ctx &c = ctx();
   const size_t n = (size_t)w * hloc;
@@ -43,8 +43,8 @@ void mgpu_fill_f64_band(const rdb200_comm *comm, double *d_band, int w, int hloc
 }
 
 // pit_mask<D8 / D4>: the float32 band mask on the key band, with kappa_G(nodata)
-void mgpu_pit_mask_f64_band(const rdb200_comm *comm, const double *d_band, uint8_t *d_mask, int w, int hloc, double nodata, int gt,
-                            int gb, int row0, int H, bool topo4) {
+void mgpu_pit_mask_band(const rdb200_comm *comm, const double *d_band, uint8_t *d_mask, int w, int hloc, double nodata, int gt,
+                        int gb, int row0, int H, bool topo4) {
   check_mask_band("mgpu_pit_mask", comm, d_band, w, hloc, gt, gb, row0, H);
   if (!d_mask) fail("mgpu_pit_mask: null pointer");
   DevBuf<float> k(static_cast<size_t>(w) * hloc);
@@ -54,8 +54,8 @@ void mgpu_pit_mask_f64_band(const rdb200_comm *comm, const double *d_band, uint8
 
 // HasDepressions<D8 / D4>: strict pits of the doubles first (no keys needed), as the float32 driver does; only if no
 // rank finds one, kappa_G, the band fill on the keys and the compare of the owned rows
-bool mgpu_has_depressions_f64_band(const rdb200_comm *comm, const double *d_band, int w, int hloc, int gt, int gb, int row0, int H,
-                                   bool topo4) {
+bool mgpu_has_depressions_band(const rdb200_comm *comm, const double *d_band, int w, int hloc, int gt, int gb, int row0, int H,
+                               bool topo4) {
   check_mask_band("mgpu_has_depressions", comm, d_band, w, hloc, gt, gb, row0, H);
   Ctx &c = ctx();
   gt = gt ? 1 : 0;
@@ -67,7 +67,7 @@ bool mgpu_has_depressions_f64_band(const rdb200_comm *comm, const double *d_band
     DevBuf<double> z(n);
     RDB_CK(cudaMemcpyAsync(z.p, d_band, n * sizeof(double), cudaMemcpyDeviceToDevice, c.stream));
     exchange_band_rows(comm, z.p, sizeof(double), w, hloc, gt, gb);
-    strict_pit_f64_dev(z.p, w, hloc, topo4, flag.p);
+    strict_pit_dev(z.p, w, hloc, topo4, flag.p);
   }
   comm_allreduce(comm, flag.p, 1, RDB200_MAX_I32);
   if (read_i32(flag.p)) return true;
@@ -83,8 +83,8 @@ bool mgpu_has_depressions_f64_band(const rdb200_comm *comm, const double *d_band
 
 // ResolveFlatsEpsilon: the float32 band flats on kappa_G return the increment mask, which the owned doubles take as
 // ulps; then one exchange puts the neighbours' resolved edge rows in the ghost rows, as the float32 call leaves them
-void mgpu_resolve_flats_f64_band(const rdb200_comm *comm, double *d_band, int w, int hloc, double nodata, int gt, int gb,
-                                 int *seam_iters) {
+void mgpu_resolve_flats_band(const rdb200_comm *comm, double *d_band, int w, int hloc, double nodata, int gt, int gb,
+                             int *seam_iters) {
   check_band_args("mgpu_resolve_flats", comm, d_band, w, hloc, gt, gb);
   Ctx &c = ctx();
   const size_t n = (size_t)w * hloc;
@@ -102,8 +102,8 @@ void mgpu_resolve_flats_f64_band(const rdb200_comm *comm, double *d_band, int w,
 // float32 band protocol on kappa_G, and then either d8_flow_flats (alter = 0) or the float steps of d8_flats_alter_dem on
 // the owned rows, one exchange of the altered edge rows and the directions of the doubles again (alter = 1).  On return
 // the ghost rows of d_dirs (and, with alter = 1, of d_band) hold the neighbours' edge rows, as in the float32 driver.
-void mgpu_d8_flow_directions_flats_f64_band(const rdb200_comm *comm, double *d_band, uint8_t *d_dirs, int w, int hloc, double nodata,
-                                            int gt, int gb, bool alter, int *seam_iters) {
+void mgpu_d8_flow_directions_flats_band(const rdb200_comm *comm, double *d_band, uint8_t *d_dirs, int w, int hloc, double nodata,
+                                        int gt, int gb, bool alter, int *seam_iters) {
   const char *what = "mgpu_d8_flow_directions_flats";
   if (!d_dirs) fail("%s: null pointer", what);
   check_band_args(what, comm, d_band, w, hloc, gt, gb);
@@ -113,14 +113,14 @@ void mgpu_d8_flow_directions_flats_f64_band(const rdb200_comm *comm, double *d_b
   const size_t n = (size_t)w * hloc;
   DevBuf<float> k(n);
   const float nd = mgpu_f64_keys_dev(comm, d_band, k.p, w, hloc, gt, gb, nodata, nullptr, nullptr);
-  d8_flow_directions_f64_dev(d_band, d_dirs, w, hloc, nodata);
+  d8_flow_directions_dev(d_band, d_dirs, w, hloc, nodata);
   DevBuf<int32_t> mask(alter ? n : 0);
   const int iters = mgpu_dir_flats_band(comm, k.p, d_dirs, w, hloc, nd, gt, gb, alter, alter ? mask.p : nullptr);
   k.reset();
   if (alter) {
     f64_float_steps_dev(d_band, mask.p, w, hloc);  // local rows 1 .. hloc-2: the owned rows, less the raster's edge rows
     exchange_band_rows(comm, d_band, sizeof(double), w, hloc, gt, gb);
-    d8_flow_directions_f64_dev(d_band, d_dirs, w, hloc, nodata);
+    d8_flow_directions_dev(d_band, d_dirs, w, hloc, nodata);
   }
   exchange_band_rows(comm, d_dirs, 1, w, hloc, gt, gb);
   RDB_CK(cudaStreamSynchronize(c.stream));
@@ -130,8 +130,8 @@ void mgpu_d8_flow_directions_flats_f64_band(const rdb200_comm *comm, double *d_b
 // FlowAccumulation of a double band.  Methods 0 (D8) and 2 (D4) compare elevations only: the float32 band accumulation
 // on kappa_G.  The others compute with them: the double flow metric on a copy of the band whose ghost rows hold the
 // neighbours' edge rows, then the band accumulation of those proportions.  The caller's ghost rows are not read.
-void mgpu_fa_f64_band(const rdb200_comm *comm, const double *d_dem, double *d_accum, int w, int hloc, double nodata, int gt, int gb,
-                      int method, double xparam, bool ones, int *xrounds) {
+void mgpu_fa_band(const rdb200_comm *comm, const double *d_dem, double *d_accum, int w, int hloc, double nodata, int gt, int gb,
+                  int method, double xparam, bool ones, int *xrounds) {
   Ctx &c = ctx();
   const size_t n = (size_t)w * hloc;
   if (method == 0 || method == 2) {
@@ -145,7 +145,7 @@ void mgpu_fa_f64_band(const rdb200_comm *comm, const double *d_dem, double *d_ac
     DevBuf<double> z(n);
     RDB_CK(cudaMemcpyAsync(z.p, d_dem, n * sizeof(double), cudaMemcpyDeviceToDevice, c.stream));
     exchange_band_rows(comm, z.p, sizeof(double), w, hloc, gt, gb);
-    fm_method_f64_dev(method, z.p, props.p, w, hloc, nodata, xparam);
+    fm_method_dev(method, z.p, props.p, w, hloc, nodata, xparam);
   }
   if (ones) {
     const size_t want = (n + 255) / 256, cap = (size_t)c.num_sms * 8;

@@ -222,7 +222,7 @@ void d8_flow_directions_dev(const float *d_dem, uint8_t *d_dirs, int w, int h, f
 }
 
 // the same rule on doubles, compared as doubles (one 8 B load per cell and neighbour, 1 B out)
-void d8_flow_directions_f64_dev(const double *d_dem, uint8_t *d_dirs, int w, int h, double nodata) {
+void d8_flow_directions_dev(const double *d_dem, uint8_t *d_dirs, int w, int h, double nodata) {
   Ctx &c = ctx();
   dim3 blk(128), grd((w + 127) / 128, h < 16384 ? h : 16384);
   d8_flowdirs_kernel<double><<<grd, blk, 0, c.stream>>>(d_dem, d_dirs, w, h, nodata);
@@ -240,25 +240,8 @@ static void fm_launch(const T *d_dem, float *d_props, int w, int h, T nodata, do
   count_launch();
 }
 
-void fm_d8_dev(const float *d_dem, float *d_props, int w, int h, float nodata) {
-  fm_launch<FM_MODE_D8>(d_dem, d_props, w, h, nodata, 0.0);
-}
-void fm_tarboton_dev(const float *d_dem, float *d_props, int w, int h, float nodata) {
-  fm_launch<FM_MODE_DINF>(d_dem, d_props, w, h, nodata, 0.0);
-}
-void fm_d4_dev(const float *d_dem, float *d_props, int w, int h, float nodata) {
-  fm_launch<FM_MODE_D4>(d_dem, d_props, w, h, nodata, 0.0);
-}
-void fm_holmgren_dev(const float *d_dem, float *d_props, int w, int h, float nodata, double xparam) {
-  fm_launch<FM_MODE_HOLMGREN>(d_dem, d_props, w, h, nodata, xparam);
-}
-void fm_freeman_dev(const float *d_dem, float *d_props, int w, int h, float nodata, double xparam) {
-  fm_launch<FM_MODE_FREEMAN>(d_dem, d_props, w, h, nodata, xparam);
-}
-
-// the same five metrics on doubles (reference templates with E = double), by the C ABI's method number:
-// 0 FM_D8, 1 FM_Tarboton, 2 FM_D4, 3 FM_Holmgren (FM_Quinn = exponent 1), 4 FM_Freeman
-void fm_method_f64_dev(int method, const double *d_dem, float *d_props, int w, int h, double nodata, double xparam) {
+template <class T>
+void fm_method_dev(int method, const T *d_dem, float *d_props, int w, int h, T nodata, double xparam) {
   switch (method) {
     case 0: fm_launch<FM_MODE_D8>(d_dem, d_props, w, h, nodata, 0.0); break;
     case 1: fm_launch<FM_MODE_DINF>(d_dem, d_props, w, h, nodata, 0.0); break;
@@ -268,5 +251,7 @@ void fm_method_f64_dev(int method, const double *d_dem, float *d_props, int w, i
     default: fail("unknown flow metric %d", method);
   }
 }
+template void fm_method_dev(int, const float *, float *, int, int, float, double);
+template void fm_method_dev(int, const double *, float *, int, int, double, double);  // reference templates with E = double
 
 }  // namespace rdb

@@ -309,30 +309,17 @@ def fill_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, solver_cls=None
         if not cxx:
             raise ValueError("fill_band: float64 bands run in the C++ band driver only; the Python band protocol "
                              "(solver_cls, RDB_BAND_DRIVER=python) takes float32")
-        return _fill_band_f64(local_dem, g_top, g_bot, group, return_stats, row0, height, topology)
-    if topology == "D4" and not cxx:
+    elif topology == "D4" and not cxx:
         raise ValueError("fill_band(topology='D4') runs in the C++ band driver only; the Python band protocol "
                          "(solver_cls, RDB_BAND_DRIVER=python) fills with D8")
     if cxx:
         # the product path: the whole band protocol (multigrid start, halo exchanges, V-cycle corrections, termination)
         # runs in C++ over the library's communicator (csrc/fill.cu: mgpu_fill_band); in place on local_dem
-        from . import _lib
-        assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
-        _lib.use_torch_stream()
+        _lib, fn, cm = _band_driver(local_dem, f"fill_depressions_{topology.lower()}_{{}}", group)
+        row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
         h_, w_ = local_dem.shape
-        if height <= 0:
-            hh = torch.tensor([h_ - g_top - g_bot], dtype=torch.int64, device=local_dem.device)
-            if world > 1:
-                allh = [torch.zeros_like(hh) for _ in range(world)]
-                dist.all_gather(allh, hh, group=group)
-                height = int(sum(int(t.item()) for t in allh))
-                row0 = int(sum(int(t.item()) for t in allh[:rank])) - g_top
-            else:
-                height, row0 = h_, 0
         xr = C.c_int32(0)
-        cm = lib_comm(group, local_dem.is_cuda)
-        fn = _lib.lib().rdb200_mgpu_fill_depressions_d8_f32 if topology == "D8" else _lib.lib().rdb200_mgpu_fill_depressions_d4_f32
-        _lib.check(fn(cm.handle, local_dem.data_ptr(), w_, h_, int(g_top), int(g_bot), int(row0), int(height), C.byref(xr)))
+        _lib.check(fn(cm.handle, local_dem.data_ptr(), w_, h_, int(g_top), int(g_bot), row0, height, C.byref(xr)))
         if return_stats:
             return local_dem, int(xr.value), _lib.stats()
         return local_dem, int(xr.value)
@@ -374,18 +361,12 @@ def pit_mask_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: flo
     are not read.  ``row0`` / ``height`` as in :func:`fill_band` (gathered from the ranks when ``height`` <= 0).
     Collective.  Returns the uint8 mask of the local shape whose owned rows are the single-GPU bits (ghost rows
     unspecified).  A float64 band gives the bits of :func:`richdem_b200.f64` on the whole raster."""
-    from . import _lib
     if topology not in ("D8", "D4"):
         raise Exception("Unknown topology!")
-    if _is_f64(local_dem):
-        return _pit_mask_band_f64(local_dem, g_top, g_bot, nodata, topology, row0, height, group)
-    assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
+    _lib, fn, cm = _band_driver(local_dem, f"pit_mask_{topology.lower()}_{{}}", group)
     row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
-    _lib.use_torch_stream()
     h, w = local_dem.shape
     mask = torch.empty((h, w), dtype=torch.uint8, device=local_dem.device)
-    cm = lib_comm(group, local_dem.is_cuda)
-    fn = _lib.lib().rdb200_mgpu_pit_mask_d8_f32 if topology == "D8" else _lib.lib().rdb200_mgpu_pit_mask_d4_f32
     _lib.check(fn(cm.handle, local_dem.data_ptr(), mask.data_ptr(), w, h, float(nodata), int(g_top), int(g_bot), row0, height))
     return mask
 
@@ -395,18 +376,12 @@ def has_depressions_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, topo
     """HasDepressions of the whole raster, from this rank's band (arguments as :func:`pit_mask_band`).  A strict pit in any
     band answers after one all-reduce; the band fill runs only when there is none.  Collective; every rank gets the
     same answer.  Float64 bands too."""
-    from . import _lib
     if topology not in ("D8", "D4"):
         raise Exception("Unknown topology!")
-    if _is_f64(local_dem):
-        return _has_depressions_band_f64(local_dem, g_top, g_bot, topology, row0, height, group)
-    assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
+    _lib, fn, cm = _band_driver(local_dem, f"has_depressions_{topology.lower()}_{{}}", group)
     row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
-    _lib.use_torch_stream()
     h, w = local_dem.shape
     out = C.c_int32(0)
-    cm = lib_comm(group, local_dem.is_cuda)
-    fn = _lib.lib().rdb200_mgpu_has_depressions_d8_f32 if topology == "D8" else _lib.lib().rdb200_mgpu_has_depressions_d4_f32
     _lib.check(fn(cm.handle, local_dem.data_ptr(), w, h, int(g_top), int(g_bot), row0, height, C.byref(out)))
     return bool(out.value)
 
@@ -559,23 +534,18 @@ def fa_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: float, di
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     mid, xparam = fa_method_id(method, exponent, dinf)
     import os
-    if _is_f64(local_dem):
-        if accumulator_cls is not None or os.environ.get("RDB_BAND_DRIVER", "cxx") == "python":
-            raise ValueError("fa_band: float64 bands run in the C++ band driver only; the Python band protocol "
-                             "(accumulator_cls, RDB_BAND_DRIVER=python) takes float32")
-        return _fa_band_f64(local_dem, g_top, g_bot, nodata, weights, group, return_stats, mid, xparam)
-    if accumulator_cls is None and os.environ.get("RDB_BAND_DRIVER", "cxx") != "python":
-        from . import _lib
+    cxx = accumulator_cls is None and os.environ.get("RDB_BAND_DRIVER", "cxx") != "python"
+    if _is_f64(local_dem) and not cxx:
+        raise ValueError("fa_band: float64 bands run in the C++ band driver only; the Python band protocol "
+                         "(accumulator_cls, RDB_BAND_DRIVER=python) takes float32")
+    if cxx:
+        _lib, fn, cm = _band_driver(local_dem, "fa_method_{}_f64", group)
         ones = weights is None
         acc = torch.empty(local_dem.shape, dtype=torch.float64, device=local_dem.device) if ones else weights
-        assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
         assert _on_device(acc) and acc.dtype == torch.float64 and acc.is_contiguous()
-        _lib.use_torch_stream()
         xr = C.c_int32(0)
-        cm = lib_comm(group, local_dem.is_cuda)
-        _lib.check(_lib.lib().rdb200_mgpu_fa_method_f32_f64(cm.handle, local_dem.data_ptr(), acc.data_ptr(), local_dem.shape[1],
-                                                            local_dem.shape[0], float(nodata), int(g_top), int(g_bot), mid,
-                                                            xparam, int(ones), C.byref(xr)))
+        _lib.check(fn(cm.handle, local_dem.data_ptr(), acc.data_ptr(), local_dem.shape[1], local_dem.shape[0], float(nodata),
+                      int(g_top), int(g_bot), mid, xparam, int(ones), C.byref(xr)))
         if return_stats:
             return acc, int(xr.value), _lib.stats()
         return acc, int(xr.value)
@@ -820,16 +790,10 @@ def resolve_flats_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata
     number of seam iterations (flags + heights).  The protocol runs in C++ over the library's
     communicator (csrc/flats.cu: mgpu_resolve_flats_band).  A float64 band takes its increments as double ulps and
     its ghost rows are not read on entry."""
-    from . import _lib
-    if _is_f64(local_dem):
-        return _resolve_flats_band_f64(local_dem, g_top, g_bot, nodata, group)
-    assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
-    _lib.use_torch_stream()
+    _lib, fn, cm = _band_driver(local_dem, "resolve_flats_epsilon_{}", group)
     h, w = local_dem.shape
     it = C.c_int32(0)
-    cm = lib_comm(group, local_dem.is_cuda)
-    _lib.check(_lib.lib().rdb200_mgpu_resolve_flats_epsilon_f32(cm.handle, local_dem.data_ptr(), w, h, float(nodata), int(g_top),
-                                                                int(g_bot), C.byref(it)))
+    _lib.check(fn(cm.handle, local_dem.data_ptr(), w, h, float(nodata), int(g_top), int(g_bot), C.byref(it)))
     return int(it.value)
 
 
@@ -843,18 +807,12 @@ def d8_flow_directions_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, n
     the owned rows in place, as on one GPU.  Collective.  Returns (uint8 directions of the same local shape, whose ghost
     rows hold the neighbours' edge-row directions, seam iterations).  A float64 band takes its directions from the doubles
     and, with ``alter=True``, the reference's float steps (:func:`richdem_b200.f64.FlowDirectionsD8Resolved`)."""
-    from . import _lib
-    if _is_f64(local_dem):
-        return _d8_flow_directions_band_f64(local_dem, g_top, g_bot, nodata, alter, group)
-    assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
-    _lib.use_torch_stream()
+    _lib, fn, cm = _band_driver(local_dem, "d8_flow_directions_flats_{}", group)
     h, w = local_dem.shape
     dirs = torch.empty((h, w), dtype=torch.uint8, device=local_dem.device)
     it = C.c_int32(0)
-    cm = lib_comm(group, local_dem.is_cuda)
-    _lib.check(_lib.lib().rdb200_mgpu_d8_flow_directions_flats_f32(cm.handle, local_dem.data_ptr(), dirs.data_ptr(), w, h,
-                                                                   float(nodata), int(g_top), int(g_bot), int(bool(alter)),
-                                                                   C.byref(it)))
+    _lib.check(fn(cm.handle, local_dem.data_ptr(), dirs.data_ptr(), w, h, float(nodata), int(g_top), int(g_bot),
+                  int(bool(alter)), C.byref(it)))
     return dirs, int(it.value)
 
 
@@ -883,17 +841,11 @@ def flow_proportions_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nod
     here with the neighbours' edge rows.  ``method`` / ``exponent`` and their errors are those of
     :func:`richdem_b200.FlowProportions`.  Collective.  Returns float32 proportions of shape (local rows, W, 9) whose owned
     rows are the single-GPU bits (ghost rows scratch)."""
-    from . import _lib
     mid, xparam = _method_id(method, exponent, "FlowProportions")
-    if _is_f64(local_dem):
-        return _flow_proportions_band_f64(local_dem, g_top, g_bot, nodata, mid, xparam, group)
-    assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
-    _lib.use_torch_stream()
+    _lib, fn, cm = _band_driver(local_dem, "fm_method_{}", group)
     h, w = local_dem.shape
     props = torch.empty((h, w, 9), dtype=torch.float32, device=local_dem.device)
-    cm = lib_comm(group, local_dem.is_cuda)
-    _lib.check(_lib.lib().rdb200_mgpu_fm_method_f32(cm.handle, mid, local_dem.data_ptr(), props.data_ptr(), w, h, float(nodata),
-                                                    int(g_top), int(g_bot), xparam))
+    _lib.check(fn(cm.handle, mid, local_dem.data_ptr(), props.data_ptr(), w, h, float(nodata), int(g_top), int(g_bot), xparam))
     return props
 
 
@@ -929,136 +881,44 @@ def terrain_attribute_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, at
     here with the neighbours' edge rows.  ``attrib`` and its error are those of :func:`richdem_b200.TerrainAttribute`;
     ``cell_x`` / ``cell_y`` are the cell lengths, |geotransform[1]| and |geotransform[5]|.  Collective.  Returns the
     float32 attribute of the local shape, NoData -9999, whose owned rows are the single-GPU bits (ghost rows scratch)."""
-    from . import _lib, _terrain_attrib_id
+    from . import _terrain_attrib_id
     aid = _terrain_attrib_id(attrib)
-    if _is_f64(local_dem):
-        return _terrain_attribute_band_f64(local_dem, g_top, g_bot, aid, nodata, zscale, cell_x, cell_y, group)
-    assert _on_device(local_dem) and local_dem.dtype == torch.float32 and local_dem.is_contiguous()
-    _lib.use_torch_stream()
+    _lib, fn, cm = _band_driver(local_dem, "terrain_attribute_{}", group)
     h, w = local_dem.shape
     out = torch.empty((h, w), dtype=torch.float32, device=local_dem.device)
-    cm = lib_comm(group, local_dem.is_cuda)
-    _lib.check(_lib.lib().rdb200_mgpu_terrain_attribute_f32(cm.handle, aid, local_dem.data_ptr(), out.data_ptr(), w, h,
-                                                            float(nodata), -9999.0, float(zscale), float(cell_x), float(cell_y),
-                                                            int(g_top), int(g_bot)))
+    _lib.check(fn(cm.handle, aid, local_dem.data_ptr(), out.data_ptr(), w, h, float(nodata), -9999.0, float(zscale),
+                  float(cell_x), float(cell_y), int(g_top), int(g_bot)))
     return out
 
 
 # =================================================================================================
-# float64 bands: the C++ band drivers on float keys every band shares (csrc/f64.cu: kappa_G), and the double flow
-# metrics and attributes (csrc/f64_band.cu).  NoData is a double.
+# The C++ band drivers by element type: float32 bands, and float64 bands, which run the float32 drivers on float keys
+# every band shares (csrc/f64.cu: kappa_G) and the double flow metrics and attributes (csrc/f64_band.cu).  NoData is a
+# double.
 # =================================================================================================
 def _is_f64(t) -> bool:
     return torch is not None and isinstance(t, torch.Tensor) and t.dtype == torch.float64
 
 
-def _f64_band(local_dem):
+def _band_driver(local_dem, name: str, group):
+    """(_lib, rdb200_mgpu_<name> with {} the band's element type f32 / f64, the library's communicator for ``group``),
+    with the library on torch's current stream."""
     from . import _lib
-    assert _on_device(local_dem) and local_dem.dtype == torch.float64 and local_dem.is_contiguous()
+    f64 = _is_f64(local_dem)
+    assert _on_device(local_dem) and local_dem.dtype == (torch.float64 if f64 else torch.float32) and local_dem.is_contiguous()
     _lib.use_torch_stream()
-    return _lib, _lib.lib()
-
-
-def _fill_band_f64(local_dem, g_top, g_bot, group, return_stats, row0, height, topology):
-    _lib, L = _f64_band(local_dem)
-    row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
-    h, w = local_dem.shape
-    xr = C.c_int32(0)
-    cm = lib_comm(group, local_dem.is_cuda)
-    fn = L.rdb200_mgpu_fill_depressions_d8_f64 if topology == "D8" else L.rdb200_mgpu_fill_depressions_d4_f64
-    _lib.check(fn(cm.handle, local_dem.data_ptr(), w, h, int(g_top), int(g_bot), row0, height, C.byref(xr)))
-    if return_stats:
-        return local_dem, int(xr.value), _lib.stats()
-    return local_dem, int(xr.value)
-
-
-def _pit_mask_band_f64(local_dem, g_top, g_bot, nodata, topology, row0, height, group):
-    _lib, L = _f64_band(local_dem)
-    row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
-    h, w = local_dem.shape
-    mask = torch.empty((h, w), dtype=torch.uint8, device=local_dem.device)
-    cm = lib_comm(group, local_dem.is_cuda)
-    fn = L.rdb200_mgpu_pit_mask_d8_f64 if topology == "D8" else L.rdb200_mgpu_pit_mask_d4_f64
-    _lib.check(fn(cm.handle, local_dem.data_ptr(), mask.data_ptr(), w, h, float(nodata), int(g_top), int(g_bot), row0, height))
-    return mask
-
-
-def _has_depressions_band_f64(local_dem, g_top, g_bot, topology, row0, height, group):
-    _lib, L = _f64_band(local_dem)
-    row0, height = _band_geometry(local_dem, g_top, g_bot, row0, height, group)
-    h, w = local_dem.shape
-    out = C.c_int32(0)
-    cm = lib_comm(group, local_dem.is_cuda)
-    fn = L.rdb200_mgpu_has_depressions_d8_f64 if topology == "D8" else L.rdb200_mgpu_has_depressions_d4_f64
-    _lib.check(fn(cm.handle, local_dem.data_ptr(), w, h, int(g_top), int(g_bot), row0, height, C.byref(out)))
-    return bool(out.value)
-
-
-def _resolve_flats_band_f64(local_dem, g_top, g_bot, nodata, group):
-    _lib, L = _f64_band(local_dem)
-    h, w = local_dem.shape
-    it = C.c_int32(0)
-    cm = lib_comm(group, local_dem.is_cuda)
-    _lib.check(L.rdb200_mgpu_resolve_flats_epsilon_f64(cm.handle, local_dem.data_ptr(), w, h, float(nodata), int(g_top),
-                                                       int(g_bot), C.byref(it)))
-    return int(it.value)
-
-
-def _d8_flow_directions_band_f64(local_dem, g_top, g_bot, nodata, alter, group):
-    _lib, L = _f64_band(local_dem)
-    h, w = local_dem.shape
-    dirs = torch.empty((h, w), dtype=torch.uint8, device=local_dem.device)
-    it = C.c_int32(0)
-    cm = lib_comm(group, local_dem.is_cuda)
-    _lib.check(L.rdb200_mgpu_d8_flow_directions_flats_f64(cm.handle, local_dem.data_ptr(), dirs.data_ptr(), w, h, float(nodata),
-                                                          int(g_top), int(g_bot), int(bool(alter)), C.byref(it)))
-    return dirs, int(it.value)
-
-
-def _fa_band_f64(local_dem, g_top, g_bot, nodata, weights, group, return_stats, mid, xparam):
-    _lib, L = _f64_band(local_dem)
-    ones = weights is None
-    acc = torch.empty(local_dem.shape, dtype=torch.float64, device=local_dem.device) if ones else weights
-    assert _on_device(acc) and acc.dtype == torch.float64 and acc.is_contiguous()
-    xr = C.c_int32(0)
-    cm = lib_comm(group, local_dem.is_cuda)
-    _lib.check(L.rdb200_mgpu_fa_method_f64_f64(cm.handle, local_dem.data_ptr(), acc.data_ptr(), local_dem.shape[1],
-                                               local_dem.shape[0], float(nodata), int(g_top), int(g_bot), mid, xparam, int(ones),
-                                               C.byref(xr)))
-    if return_stats:
-        return acc, int(xr.value), _lib.stats()
-    return acc, int(xr.value)
-
-
-def _flow_proportions_band_f64(local_dem, g_top, g_bot, nodata, mid, xparam, group):
-    _lib, L = _f64_band(local_dem)
-    h, w = local_dem.shape
-    props = torch.empty((h, w, 9), dtype=torch.float32, device=local_dem.device)
-    cm = lib_comm(group, local_dem.is_cuda)
-    _lib.check(L.rdb200_mgpu_fm_method_f64(cm.handle, mid, local_dem.data_ptr(), props.data_ptr(), w, h, float(nodata),
-                                           int(g_top), int(g_bot), xparam))
-    return props
-
-
-def _terrain_attribute_band_f64(local_dem, g_top, g_bot, aid, nodata, zscale, cell_x, cell_y, group):
-    _lib, L = _f64_band(local_dem)
-    h, w = local_dem.shape
-    out = torch.empty((h, w), dtype=torch.float32, device=local_dem.device)
-    cm = lib_comm(group, local_dem.is_cuda)
-    _lib.check(L.rdb200_mgpu_terrain_attribute_f64(cm.handle, aid, local_dem.data_ptr(), out.data_ptr(), w, h, float(nodata),
-                                                   -9999.0, float(zscale), float(cell_x), float(cell_y), int(g_top), int(g_bot)))
-    return out
+    return _lib, getattr(_lib.lib(), "rdb200_mgpu_" + name.format("f64" if f64 else "f32")), lib_comm(group, local_dem.is_cuda)
 
 
 def f64_order_keys_band(local_dem: "torch.Tensor", g_top: int, g_bot: int, nodata: float, group=None):
     """Diagnostic (not a stable interface): kappa_G, the float keys the float64 band drivers run the float32 engines on.
     Collective.  Returns (float32 keys of the local shape, whose ghost rows hold the neighbours' keys, kappa_G(nodata),
     True for global ranks / False for the cast to float)."""
-    _lib, L = _f64_band(local_dem)
+    assert _is_f64(local_dem)
+    _lib, fn, cm = _band_driver(local_dem, "f64_order_keys", group)
     h, w = local_dem.shape
     keys = torch.empty((h, w), dtype=torch.float32, device=local_dem.device)
     nd, ranked = C.c_float(0), C.c_int32(0)
-    cm = lib_comm(group, local_dem.is_cuda)
-    _lib.check(L.rdb200_mgpu_f64_order_keys(cm.handle, local_dem.data_ptr(), keys.data_ptr(), w, h, float(nodata), int(g_top),
-                                            int(g_bot), C.byref(nd), C.byref(ranked)))
+    _lib.check(fn(cm.handle, local_dem.data_ptr(), keys.data_ptr(), w, h, float(nodata), int(g_top), int(g_bot), C.byref(nd),
+                  C.byref(ranked)))
     return keys, float(nd.value), bool(ranked.value)
