@@ -94,6 +94,20 @@ RDB200_API int rdb200_fill_depressions_d8_f32(float *dem, int32_t width, int32_t
  *   Same engine with the 4-neighbour stencil; bit-identical. */
 RDB200_API int rdb200_fill_depressions_d4_f32(float *dem, int32_t width, int32_t height);
 
+/* richdem::PriorityFloodEpsilon_Barnes2014<Topology::D8 / D4>(Array2D<float>&) -- FillDepressions(epsilon=True)
+ *   include/richdem/depressions/Barnes2014.hpp:336-420 (pyrichdem: rdPFepsilonD8 / rdPFepsilonD4, pywrapper.hpp:34-35).
+ *   In place.  With up(x) = nextafterf(x, +inf), the result W is the unique solution of
+ *       W(c) = Z(c)                                               on the raster's border and where Z(c) == nodata,
+ *       W(c) = max(Z(c), min over the neighbours n of up(W(n)))   elsewhere (8 neighbours for D8, 4 for D4).
+ *   NoData cells are never raised and offer up(nodata) to their neighbours; a NaN nodata pins nothing; NaN elevations are
+ *   not supported.  The reference's result depends on the order in which its priority queue breaks ties, so this is NOT
+ *   bit-identical to it: W is order-free and never above the reference's surface anywhere (on NoData-free rasters a few
+ *   ulps below it in under 1 % of cells; next to NoData cells inside depressions it can be lower by more).  Without NoData
+ *   every interior cell of W has a strictly lower neighbour, so W has no depressions and no flats.
+ *   Stats: fill_rounds, fill_tile_visits. */
+RDB200_API int rdb200_fill_depressions_epsilon_d8_f32(float *dem, int32_t width, int32_t height, float nodata);
+RDB200_API int rdb200_fill_depressions_epsilon_d4_f32(float *dem, int32_t width, int32_t height, float nodata);
+
 /* richdem::pit_mask<Topology::D8 / D4>(const Array2D<float>&, Array2D<uint8_t>&)
  *   include/richdem/depressions/Barnes2014.hpp:593-676 (app rd_depressions_mask).  mask (width x height, written in
  *   full): 3 where dem == nodata, 1 where the cell lies below the depression-filled surface of dem (the fill above,
@@ -300,6 +314,10 @@ RDB200_API int rdb200_terrain_attribute_f64(int32_t attribute, const double *dem
  * d_dem are unspecified. */
 RDB200_API int rdb200_dev_fill_depressions_d8_f32(float *d_dem, int32_t width, int32_t height);
 RDB200_API int rdb200_dev_fill_depressions_d4_f32(float *d_dem, int32_t width, int32_t height);
+/* The epsilon fill of rdb200_fill_depressions_epsilon_d8_f32 / _d4_f32 in place, with the same contract (never above the
+ * reference's surface, not bit-identical to it) and the same rule for d_dem while the call runs. */
+RDB200_API int rdb200_dev_fill_depressions_epsilon_d8_f32(float *d_dem, int32_t width, int32_t height, float nodata);
+RDB200_API int rdb200_dev_fill_depressions_epsilon_d4_f32(float *d_dem, int32_t width, int32_t height, float nodata);
 /* pit_mask / HasDepressions on device pointers (d_dem is not modified; *out is a host int) */
 RDB200_API int rdb200_dev_pit_mask_d8_f32(const float *d_dem, uint8_t *d_mask, int32_t width, int32_t height, float nodata);
 RDB200_API int rdb200_dev_pit_mask_d4_f32(const float *d_dem, uint8_t *d_mask, int32_t width, int32_t height, float nodata);

@@ -45,6 +45,16 @@ template <class A2>
 void fill_depressions_d4(A2 &dem) {
   check(rdb200_fill_depressions_d4_f32(dem.data(), dem.width(), dem.height()));
 }
+// FillDepressions(epsilon=True): the order-free surface of rdb200_fill_depressions_epsilon_d8_f32 (never above the
+// reference's PriorityFloodEpsilon_Barnes2014, not bit-identical to it); cells equal to dem.noData() are pinned
+template <class A2>
+void fill_depressions_epsilon_d8(A2 &dem) {
+  check(rdb200_fill_depressions_epsilon_d8_f32(dem.data(), dem.width(), dem.height(), (float)dem.noData()));
+}
+template <class A2>
+void fill_depressions_epsilon_d4(A2 &dem) {
+  check(rdb200_fill_depressions_epsilon_d4_f32(dem.data(), dem.width(), dem.height(), (float)dem.noData()));
+}
 template <class A2>
 void resolve_flats_epsilon(A2 &dem) {
   check(rdb200_resolve_flats_epsilon_f32(dem.data(), dem.width(), dem.height(), (float)dem.noData()));
@@ -516,6 +526,22 @@ RICHDEM_B200_TA64(TA_planform_curvature, RDB200_TA_PLANFORM_CURVATURE)
 RICHDEM_B200_TA64(TA_profile_curvature, RDB200_TA_PROFILE_CURVATURE)
 #undef RICHDEM_B200_TA64
 #endif  // RICHDEM_B200_F64
+
+#ifdef RICHDEM_B200_EPSILON
+// the epsilon fill (opt-in: `#define RICHDEM_B200_EPSILON` before this include), depressions/Barnes2014.hpp:336-420, also
+// reached through FillDepressionsEpsilon<topo> (depressions/depressions.hpp:23).  Opt-in because the GPU's surface is
+// not the reference's bit for bit: it is the order-free one, never above the reference's and a few ulps below it in
+// rare cells (include/richdem_b200.h, rdb200_fill_depressions_epsilon_d8_f32).  Without the macro these keep the
+// reference's CPU template.
+template <>
+inline void PriorityFloodEpsilon_Barnes2014<Topology::D8, float>(Array2D<float> &elevations) {
+  richdem_b200::fill_depressions_epsilon_d8(elevations);
+}
+template <>
+inline void PriorityFloodEpsilon_Barnes2014<Topology::D4, float>(Array2D<float> &elevations) {
+  richdem_b200::fill_depressions_epsilon_d4(elevations);
+}
+#endif  // RICHDEM_B200_EPSILON
 
 }  // namespace richdem
 

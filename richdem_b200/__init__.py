@@ -108,17 +108,21 @@ class _Elem(NamedTuple):
     fa_valid: Tuple[str, ...]  # the methods FlowAccumulation lists as valid
     fa_refused: Tuple[str, ...]  # known methods FlowAccumulation refuses for this element type
     nodata_first: bool  # FlowAccumulation / FlowProportions read no_data before they check the method
+    epsilon_refusal: Optional[str]  # why FillDepressions(epsilon=True) is refused for this element type (None: it runs)
 
 
 _F32 = _Elem(np.float32, "f32", lambda nd: float(np.float32(nd)),
              "{what}: the H100 path is built for float32 elevations (got '{dtype}'); "
              "convert with dem.astype('float32') -- there is no CPU fallback for other dtypes "
              "(float64 rasters: richdem_b200.f64 computes the float64 answer).",
-             _DINF_METHODS + ("Quinn",) + _D8_METHODS + _D4_METHODS + _EXPONENT_METHODS + _OUT_OF_SCOPE_METHODS, (), False)
+             _DINF_METHODS + ("Quinn",) + _D8_METHODS + _D4_METHODS + _EXPONENT_METHODS + _OUT_OF_SCOPE_METHODS, (), False,
+             None)
 _F64 = _Elem(np.float64, "f64", float,
              "{what}: richdem_b200.f64 is built for float64 elevations (got '{dtype}'); "
              "float32 rasters go through richdem_b200 itself.",
-             _D8_METHODS + _D4_METHODS, _DINF_METHODS + ("Quinn",) + _EXPONENT_METHODS + _OUT_OF_SCOPE_METHODS, True)
+             _D8_METHODS + _D4_METHODS, _DINF_METHODS + ("Quinn",) + _EXPONENT_METHODS + _OUT_OF_SCOPE_METHODS, True,
+             "FillDepressions(epsilon=True) is not available for float64 rasters (its one-ulp steps are double ulps, which "
+             "the float engine does not hold); fill float32 rasters with richdem_b200.FillDepressions(epsilon=True)")
 
 
 def _dem(et: _Elem, dem: rdarray, what: str) -> np.ndarray:
@@ -148,15 +152,19 @@ def _check_topology(dem, topology: str) -> None:
 
 def _fill_depressions(et, dem, epsilon, in_place, topology):
     _check_topology(dem, topology)
-    if epsilon:
-        raise Exception("FillDepressions(epsilon=True) is outside the GPU hot path (SURVEY 8f-3)")
+    if epsilon and et.epsilon_refusal:
+        raise Exception(et.epsilon_refusal)
     if not in_place:
         dem = dem.copy()
     _add_analysis(dem, f"FillDepressions(dem, epsilon={epsilon})")
     d = _dem(et, dem, "FillDepressions")
     h, w = d.shape
-    fn = getattr(_lib.lib(), f"rdb200_fill_depressions_{topology.lower()}_{et.suffix}")
-    _lib.check(fn(_lib.ptr(d), w, h))
+    if epsilon:
+        fn = getattr(_lib.lib(), f"rdb200_fill_depressions_epsilon_{topology.lower()}_{et.suffix}")
+        _lib.check(fn(_lib.ptr(d), w, h, _nodata(et, dem)))
+    else:
+        fn = getattr(_lib.lib(), f"rdb200_fill_depressions_{topology.lower()}_{et.suffix}")
+        _lib.check(fn(_lib.ptr(d), w, h))
     if not in_place:
         return dem
     return None
@@ -378,7 +386,13 @@ def _flat_mask(et, dem):  # no rdarray check, in either module
 def FillDepressions(dem: rdarray, epsilon: bool = False, in_place: bool = False,
                     topology: str = "D8") -> Optional[rdarray]:
     """Fills all depressions in a DEM (reference FillDepressions, :381-422 -> PriorityFlood_Zhou2016 for ``D8``,
-    PriorityFlood_Barnes2014<D4> for ``D4``).  Returns the filled DEM unless ``in_place``."""
+    PriorityFlood_Barnes2014<D4> for ``D4``).  Returns the filled DEM unless ``in_place``.
+
+    ``epsilon=True`` (PriorityFloodEpsilon_Barnes2014) leaves every filled cell one float step above the lowest of its
+    neighbours, so the result drains without flats: the unique surface W = max(Z, min over the neighbours of
+    nextafter(W, +inf)), with the raster's border and its ``no_data`` cells pinned.  It is never above the reference's
+    result, but not bit-identical to it (the reference's depends on its queue's tie order; see
+    ``rdb200_fill_depressions_epsilon_d8_f32`` in ``include/richdem_b200.h``)."""
     return _fill_depressions(_F32, dem, epsilon, in_place, topology)
 
 

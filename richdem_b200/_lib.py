@@ -44,6 +44,10 @@ SIGNATURES = {
     "rdb200_fill_depressions_d8_f32": [_vp, _i32, _i32],
     "rdb200_fill_depressions_d4_f32": [_vp, _i32, _i32],
     "rdb200_dev_fill_depressions_d4_f32": [_vp, _i32, _i32],
+    "rdb200_fill_depressions_epsilon_d8_f32": [_vp, _i32, _i32, _f32],
+    "rdb200_fill_depressions_epsilon_d4_f32": [_vp, _i32, _i32, _f32],
+    "rdb200_dev_fill_depressions_epsilon_d8_f32": [_vp, _i32, _i32, _f32],
+    "rdb200_dev_fill_depressions_epsilon_d4_f32": [_vp, _i32, _i32, _f32],
     "rdb200_pit_mask_d8_f32": [_vp, _vp, _i32, _i32, _f32],
     "rdb200_pit_mask_d4_f32": [_vp, _vp, _i32, _i32, _f32],
     "rdb200_has_depressions_d8_f32": [_vp, _i32, _i32, C.POINTER(_i32)],

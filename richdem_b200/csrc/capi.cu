@@ -246,6 +246,13 @@ static int fill_depressions(Side side, T *dem, int32_t w, int32_t h, bool topo4)
                      [&](Arrays &a, size_t n) { fill_depressions_dev(a.inout(dem, n), w, h, topo4); });
 }
 
+// reference depressions/Barnes2014.hpp:336-420 (PriorityFloodEpsilon_Barnes2014<topo>): the order-free surface, never
+// above the reference's (DESIGN.md section 0, f3)
+static int fill_depressions_epsilon(Side side, float *dem, int32_t w, int32_t h, float nodata, bool topo4) {
+  return raster_call(side, "fill_depressions_epsilon: null dem", {dem}, w, h,
+                     [&](Arrays &a, size_t n) { fill_depressions_epsilon_dev(a.inout(dem, n), w, h, topo4, nodata); });
+}
+
 // reference depressions/Barnes2014.hpp:593-676 (pit_mask<topo>)
 template <class T>
 static int pit_mask(Side side, const T *dem, uint8_t *mask, int32_t w, int32_t h, T nodata, bool topo4) {
@@ -582,6 +589,12 @@ int rdb200_set_param(const char *name, int64_t value) {
 
 int rdb200_fill_depressions_d8_f32(float *dem, int32_t w, int32_t h) { return fill_depressions(Side::host, dem, w, h, false); }
 int rdb200_fill_depressions_d4_f32(float *dem, int32_t w, int32_t h) { return fill_depressions(Side::host, dem, w, h, true); }
+int rdb200_fill_depressions_epsilon_d8_f32(float *dem, int32_t w, int32_t h, float nodata) {
+  return fill_depressions_epsilon(Side::host, dem, w, h, nodata, false);
+}
+int rdb200_fill_depressions_epsilon_d4_f32(float *dem, int32_t w, int32_t h, float nodata) {
+  return fill_depressions_epsilon(Side::host, dem, w, h, nodata, true);
+}
 int rdb200_pit_mask_d8_f32(const float *dem, uint8_t *mask, int32_t w, int32_t h, float nodata) {
   return pit_mask(Side::host, dem, mask, w, h, nodata, false);
 }
@@ -731,6 +744,12 @@ int rdb200_dev_fill_depressions_d8_f32(float *d_dem, int32_t w, int32_t h) {
 }
 int rdb200_dev_fill_depressions_d4_f32(float *d_dem, int32_t w, int32_t h) {
   return fill_depressions(Side::device, d_dem, w, h, true);
+}
+int rdb200_dev_fill_depressions_epsilon_d8_f32(float *d_dem, int32_t w, int32_t h, float nodata) {
+  return fill_depressions_epsilon(Side::device, d_dem, w, h, nodata, false);
+}
+int rdb200_dev_fill_depressions_epsilon_d4_f32(float *d_dem, int32_t w, int32_t h, float nodata) {
+  return fill_depressions_epsilon(Side::device, d_dem, w, h, nodata, true);
 }
 int rdb200_dev_pit_mask_d8_f32(const float *d_dem, uint8_t *d_mask, int32_t w, int32_t h, float nodata) {
   return pit_mask(Side::device, d_dem, d_mask, w, h, nodata, false);

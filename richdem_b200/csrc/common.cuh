@@ -219,6 +219,8 @@ int mgpu_relax_band(const rdb200_comm *comm, rdb200_fill_state *state, int gt, i
 // elevations, and the kernels' double instantiations where it does arithmetic on them.
 void fill_depressions_dev(float *d_dem, int w, int h, bool topo4 = false);
 void fill_depressions_dev(double *d_z, int w, int h, bool topo4 = false);
+// FillDepressions(epsilon=True) of a float raster (fill.cu): cells equal to nodata are pinned, never raised
+void fill_depressions_epsilon_dev(float *d_dem, int w, int h, bool topo4, float nodata);
 void geodesic_distance_dev(const uint8_t *d_open, int open_bit, float *d_w_inout, int w, int h);
 void geodesic_distance_pair_dev(const uint8_t *d_open, int open_bit, float *d_wa, float *d_wb, int w, int h);
 rdb200_fill_state *new_band_distance_state(const uint8_t *d_open, int open_bit, const float *d_winit, int w, int h,

@@ -213,6 +213,25 @@ __device__ __forceinline__ void enqueue_tile(const FillArgs &a, RoundCtl *next, 
 
 __device__ __forceinline__ float min3f(float a, float b, float c) { return fminf(fminf(a, b), c); }
 
+// std::nextafter(x, +inf) on the float bits: +inf (and NaN) stay, -0 goes to +denorm_min, a negative value one step
+// towards zero (-denorm_min to -0, -inf to -FLT_MAX), a positive one (and +0) one step up (FLT_MAX to +inf)
+__host__ __device__ __forceinline__ float next_up(float x) {
+  int b;
+  memcpy(&b, &x, 4);
+  b = b < 0 ? (b == (int)0x80000000 ? 1 : b - 1) : (b < 0x7f800000 ? b + 1 : b);
+  float r;
+  memcpy(&r, &b, 4);
+  return r;
+}
+
+// the neighbour term of fill_sweep_kernel<STEP>: W(c) <- min(W(c), max(Z(c), fill_step(min over the neighbours of W)))
+template <int STEP>
+__device__ __forceinline__ float fill_step(float w) {
+  if constexpr (STEP == 1) return w + 1.0f;
+  else if constexpr (STEP == 2) return next_up(w);
+  else return w;
+}
+
 // ---- the wake test (fill only) ----------------------------------------------------------------------------------------
 // A changed tile edge used to wake the neighbour across it whatever the new values were, and most of those visits found
 // nothing to do: the neighbour's cell next to the edge already sat at its Z (W == Z never moves again) or at or below
@@ -389,6 +408,9 @@ __device__ __noinline__ void fill_wake_neighbours(const FillArgs &a, const float
 // STEP = 0: depression filling,     new = min(W, max(Z, min8 W))
 // STEP = 1: geodesic distance,      new = min(W, max(Z, 1 + min8 W))   with Z = 0 on cells the flood
 //           may enter and +inf elsewhere (used for the flat-resolution gradients, csrc/flats.cu)
+// STEP = 2: epsilon fill,           new = min(W, max(Z, next_up(min8 W)))   (FillDepressions(epsilon=True); DESIGN.md
+//           3.1).  A fill in everything but the neighbour term: pinned cells, the wake test and the edge flags are the
+//           fill's (next_up(e) < W implies e < W, so the fill's wake test wakes a superset of the tiles that can drop).
 // TOPO4: the 4-neighbour (D4) stencil of FillDepressions<Topology::D4>; corner aprons are then never read
 // STAGE: round 1 of a staged lifted start (a.coarse): W is built from the coarse surface, not loaded, every row is
 //        written back, and the tile's Z is saved to a.zcopy through mapZout (a template parameter so that the later
@@ -397,6 +419,8 @@ template <int STEP, bool TOPO4 = false, bool STAGE = false>
 __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
     fill_sweep_kernel(const __grid_constant__ CUtensorMap mapW, const __grid_constant__ CUtensorMap mapZ,
                       const __grid_constant__ CUtensorMap mapZout, const __grid_constant__ FillArgs a) {
+  // a lifted start bounds the plain fill from above, not the epsilon fill (which lies higher)
+  static_assert(!(STAGE && STEP != 0), "the staged lifted round is the plain fill's");
   __shared__ __align__(128) float sW[SROWS * SP];
   __shared__ __align__(128) float sZ[TY * TX];
   __shared__ __align__(8) unsigned long long mbar;
@@ -609,7 +633,7 @@ __global__ void __launch_bounds__(FILL_THREADS, FILL_MIN_CTAS)
         atomicExch(&a.staged[t], 1);
       }
     }
-    if (STEP == 0 && WAKE_WORDS && a.edge_above) {
+    if (STEP != 1 && WAKE_WORDS && a.edge_above) {
       // (not inlined: the relaxation above keeps its registers)
       fill_wake_neighbours<TOPO4>(a, sW, sZ, t, fl, sKey, next, list_next);
       if (rowch && tid == 0) {
@@ -748,9 +772,11 @@ __global__ void __launch_bounds__(256) fill_lift_row_kernel(float *row, int W, c
 // Z = W = +inf.
 // LIFT (fill_multigrid): interior cells start at the water level of their pool x pool block in the filled max-pooled
 // raster `coarse` (an upper bound of the answer, see fill_depressions_dev) instead of +inf.
+// Cells equal to `pin` are boundary conditions too (the epsilon fill's NoData; NaN pins nothing).
 template <bool LIFT>
 __global__ void fill_init_kernel(const float *dem, float *__restrict__ Zo, float *Wo, int W, int H, int pitch, int rows,
-                                 int ox, int oy, FillDev *dev, const float *__restrict__ coarse, int Wc, int pool, int yoff) {
+                                 int ox, int oy, FillDev *dev, const float *__restrict__ coarse, int Wc, int pool, int yoff,
+                                 float pin) {
   const int px4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;  // layout column (multiple of 4)
   const float inf = __int_as_float(0x7f800000);
   float lo = inf, hi = -inf;
@@ -763,7 +789,7 @@ __global__ void fill_init_kernel(const float *dem, float *__restrict__ Zo, float
       float zz = inf, ww = inf;
       if (x >= 0 && x < W && y >= 0 && y < H) {
         zz = dem[(size_t)y * W + x];
-        const bool border = (x == 0) | (y == 0) | (x == W - 1) | (y == H - 1);
+        const bool border = (x == 0) | (y == 0) | (x == W - 1) | (y == H - 1) | (zz == pin);
         ww = border ? zz : (LIFT ? __ldg(coarse + (size_t)((y + yoff) / pool) * Wc + x / pool) : inf);
         if (zz < inf && zz > -inf) {
           lo = fminf(lo, zz);
@@ -1112,8 +1138,9 @@ struct FillState {
   float zmin = 0.f, zmax = 0.f;
   bool first_run = true;
   bool ordered = false;
-  int step_mode = 0;  // 0: fill, 1: geodesic distance
+  int step_mode = 0;  // 0: fill, 1: geodesic distance, 2: epsilon fill (fill_sweep_kernel<STEP>)
   bool topo4 = false;  // D4 fill (4-neighbour stencil)
+  float pin = __builtin_nanf("");  // cells equal to it are pinned like the raster's border (epsilon fill: NoData)
   std::vector<float> levels;
   DevBuf<FillDev> dev;
   CUtensorMap mapW, mapZ;
@@ -1215,15 +1242,15 @@ struct FillState {
         // start does not use)
       } else if (inplace) {
         dim3 grdc((W / 4 + 127) / 128, H < 2048 ? H : 2048);
-        fill_init_kernel<false><<<grdc, blk, 0, c.stream>>>(d_dem, Zc.p, Wb, W, H, W, H, 0, 0, dev.p, nullptr, 0, 1, 0);
+        fill_init_kernel<false><<<grdc, blk, 0, c.stream>>>(d_dem, Zc.p, Wb, W, H, W, H, 0, 0, dev.p, nullptr, 0, 1, 0, pin);
         count_launch();
       } else if (d_coarse) {
         fill_init_kernel<true><<<grd, blk, 0, c.stream>>>(d_dem, Zp.p, Wp.p, W, H, pitch, rows, PADL, 1, dev.p, d_coarse,
-                                                         coarse_w, coarse_k, coarse_yoff);
+                                                         coarse_w, coarse_k, coarse_yoff, pin);
         count_launch();
       } else {
         fill_init_kernel<false><<<grd, blk, 0, c.stream>>>(d_dem, Zp.p, Wp.p, W, H, pitch, rows, PADL, 1, dev.p, nullptr, 0, 1,
-                                                          0);
+                                                          0, pin);
         count_launch();
       }
       RDB_CK(cudaGetLastError());
@@ -1285,16 +1312,19 @@ struct FillState {
       mapZ = make_map(Zp.p, pitch, rows, TX, TY);
     }
     int per_sm = 0;
-    RDB_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fill_sweep_kernel<0>, FILL_THREADS, 0));
+    RDB_CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(
+        &per_sm, step_mode == 2 ? (const void *)fill_sweep_kernel<2> : (const void *)fill_sweep_kernel<0>, FILL_THREADS, 0));
     if (per_sm < 1) per_sm = 1;
     grid = c.num_sms * per_sm;
     round = 1;  // stamps start at 0, so round numbers (used as stamp values) start at 1
     // initial worklist: every tile on the perimeter of the tile grid (the only tiles whose
-    // cells can see a finite neighbour at the start)
+    // cells can see a finite neighbour at the start).  The epsilon fill pins NoData cells anywhere, and a cell whose
+    // every neighbour is pinned is lowered by no changed neighbour: every tile's first visit relaxes all of its blocks.
     std::vector<int> init;
     for (int ty = 0; ty < tilesY; ty++)
       for (int tx = 0; tx < tilesX; tx++)
-        if (d_coarse || ty == 0 || tx == 0 || ty == tilesY - 1 || tx == tilesX - 1) init.push_back(ty * tilesX + tx);
+        if (d_coarse || step_mode == 2 || ty == 0 || tx == 0 || ty == tilesY - 1 || tx == tilesX - 1)
+          init.push_back(ty * tilesX + tx);
     seed_worklist(init);
   }
 
@@ -1394,8 +1424,9 @@ struct FillState {
     a.profile = (int)c.params.fill_profile;
     a.level = __builtin_inff();
     a.dirty = dirty.p;  // null unless track_dirty() was called
-    // (the distance mode wakes every neighbour across a changed side, as the fill does with fill_wake_filter = 0)
-    a.edge_above = step_mode == 0 && c.params.fill_wake_filter != 0 ? edge_above.p : nullptr;
+    // (the distance mode wakes every neighbour across a changed side, as the fill does with fill_wake_filter = 0; the
+    // epsilon fill takes the fill's test, see fill_sweep_kernel)
+    a.edge_above = step_mode != 1 && c.params.fill_wake_filter != 0 ? edge_above.p : nullptr;
     return a;
   }
 
@@ -1426,7 +1457,9 @@ struct FillState {
       a.Z = a.coarse ? Wb : (inplace ? Zc.p : Zp.p);
       a.zcopy = a.coarse ? Zc.p : nullptr;
       const CUtensorMap &mz = a.coarse ? mapZstage : mapZ;
-      if (step_mode) fill_sweep_kernel<1><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mz, mapZ, a);
+      if (step_mode == 1) fill_sweep_kernel<1><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mz, mapZ, a);
+      else if (step_mode == 2 && topo4) fill_sweep_kernel<2, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mz, mapZ, a);
+      else if (step_mode == 2) fill_sweep_kernel<2><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mz, mapZ, a);
       else if (a.coarse && topo4) fill_sweep_kernel<0, true, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mz, mapZ, a);
       else if (a.coarse) fill_sweep_kernel<0, false, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mz, mapZ, a);
       else if (topo4) fill_sweep_kernel<0, true><<<grid, FILL_THREADS, 0, c.stream>>>(mapW, mz, mapZ, a);
@@ -2021,6 +2054,24 @@ void fill_depressions_dev(float *d_dem, int w, int h, bool topo4) {
   c.stats.cells = (int64_t)w * h;
   if (w <= 2 || h <= 2) return;  // every cell is a border cell: nothing can change
   fill_depressions_level(d_dem, w, h, 0, topo4);
+}
+
+// FillDepressions(epsilon=True): the greatest fixed point of W(c) = max(Z(c), min over the neighbours n of
+// next_up(W(n))), with W = Z on the raster border and on the cells equal to `nodata` (DESIGN.md section 0, f3).  The
+// engine relaxes it in place from +inf (fill_sweep_kernel<2>).  The multigrid start of fill_depressions_level is not
+// taken: its coarse surface is an upper bound of the plain fill, which lies below this answer.
+void fill_depressions_epsilon_dev(float *d_dem, int w, int h, bool topo4, float nodata) {
+  Ctx &c = ctx();
+  c.stats.cells = (int64_t)w * h;
+  if (w <= 2 || h <= 2) return;  // every cell is a border cell: nothing can change
+  FillState st;
+  st.step_mode = 2;
+  st.topo4 = topo4;
+  st.pin = nodata;
+  st.begin(d_dem, w, h, nullptr, 0, 0, 0, true);
+  st.run();
+  st.finish(d_dem);
+  RDB_CK(cudaStreamSynchronize(c.stream));
 }
 
 }  // namespace rdb

@@ -25,7 +25,8 @@ from . import (_F64, _fill_depressions, _flat_mask, _flow_accumulation, _flow_di
 def FillDepressions(dem: rdarray, epsilon: bool = False, in_place: bool = False,
                     topology: str = "D8") -> Optional[rdarray]:
     """FillDepressions<topo, double> (PriorityFlood_Zhou2016 for ``D8``, PriorityFlood_Barnes2014<D4> for ``D4``).
-    Returns the filled DEM unless ``in_place``; cells the fill does not raise keep their own bits."""
+    Returns the filled DEM unless ``in_place``; cells the fill does not raise keep their own bits.  ``epsilon=True`` is
+    not available for float64 rasters and raises."""
     return _fill_depressions(_F64, dem, epsilon, in_place, topology)
 
 def PitMask(dem: rdarray, topology: str = "D8") -> rdarray:
